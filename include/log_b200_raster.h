@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 16
+#define LGR_ABI_VERSION 17
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -85,15 +85,21 @@ typedef struct lgr_view {
                             SparseOptimizer consumes (sparse_optimizer.py:163-196).  Not available in band mode. */
   const int32_t* pid_map_d; /* (n) int32 or NULL: when set, point_id_pixel holds pid_map_d[row] instead of the row index of the
                             winning splat (shard mode renders received ROWS; the map turns them into global Gaussian ids) */
-  uint8_t* contrib_d;    /* (instances) uint8 or NULL, indexed like sorted_ids_d.  When set, the forward blend records per list
-                            entry which of the tile's eight 8x4 sub-tiles had a CONTRIBUTING pixel for that splat (bit w =
-                            sub-tile w), and the backward sweep walks exactly those (sub-tile, splat) pairs instead of
-                            re-testing the conservative boxes: the ~20 % of box hits that contribute nothing are never
-                            evaluated again.  Pass the same view (and buffer) to the forward and to the backward, and give
-                            the backward the forward's n_contrib_d as last_contrib_d. */
+  int32_t* contrib_id_d; /* (instances) int32 or NULL.  When set (with contrib_entry_d and contrib_count_d), the forward blend
+                            writes, per tile, the list entries that some pixel of the tile composited, compacted and in list
+                            order: tile t's k-th such entry goes to [tile_start_d[t] + k], contrib_id_d = the splat's id,
+                            contrib_entry_d = the sub-tiles that composited it (bit w = the tile's 8x4 sub-tile w) | its index
+                            in the tile list << 8; contrib_count_d[t] = the number of such entries.  The backward sweep then
+                            stages only those entries and walks exactly those (sub-tile, splat) pairs instead of re-testing
+                            the conservative boxes.  Pass the same view (and buffers) to the forward and to the backward, and
+                            give the backward the forward's n_contrib_d as last_contrib_d.  lgr_forward_render rejects
+                            (LGR_E_UNSUPPORTED) a view with a tile list of more than LGR_CONTRIB_MAX_LIST entries. */
+  uint32_t* contrib_entry_d; /* (instances) uint32 or NULL, see contrib_id_d */
+  int32_t* contrib_count_d;  /* (tiles) int32 or NULL, see contrib_id_d */
   const int32_t* last_contrib_d; /* (H,W) int32 or NULL: the n_contrib_d output of lgr_forward_render (per pixel: list index + 1 of
-                            its last contributor).  Read by lgr_backward / lgr_blend_backward together with contrib_d: a pixel
-                            is finished once the sweep has passed its last contributor (both must be set, or neither). */
+                            its last contributor).  Read by lgr_backward / lgr_blend_backward together with the contrib_*
+                            lists: a pixel is finished once the sweep has passed its last contributor (all must be set, or
+                            none). */
   const int32_t* region_count_d; /* (num_regions) int32 or NULL.  Shard mode: the rows of the call are num_regions regions of
                             region_cap rows each (rows = num_regions * region_cap) and only the first region_count_d[s] rows
                             of region s are in use (lgr_shard_layout: the counts live in the exchange buffer at off_count).
@@ -120,6 +126,7 @@ typedef struct lgr_view {
 #define LGR_SPLAT_FLOATS 12 /* per-Gaussian projected record: 3 x float4 */
 #define LGR_GRAD_FLOATS 12  /* per-Gaussian 2D-gradient accumulator: 3 x float4 */
 #define LGR_TILE_SCRATCH_INTS 33 /* per tile: one counter per 128-byte line (32 ints) + one slot of the long-tile list */
+#define LGR_CONTRIB_MAX_LIST (1 << 24) /* longest tile list whose entry indices fit lgr_view.contrib_entry_d */
 #define LGR_META_INTS 8     /* meta_d: [0]=D binned instances [1]=longest tile list [2..3]=D by the stock
                                radius-square rule (lo,hi 32 bits) [4]=#Gaussians with radius>0
                                [5]=#tiles whose list exceeds the small shared-memory sort

@@ -9,9 +9,10 @@
 // Backward: the same front-to-back walk (closed form of the published recurrence, see below).  Per contributing hit every
 // lane publishes two scalars; every 8 hits the warp contracts them against fixed per-pixel weights (pixel-coordinate
 // moments and cotangent-weighted sums) on the tensor cores (mma.sync m16n8k8, split TF32 = fp32 accuracy); the moments
-// become gradients once per staged splat, then 3 vector atomics per splat.  With View::contrib the forward records which
-// sub-tiles composited each list entry and the backward (REC) walks exactly those pairs, stopping every pixel after its
-// last contributor (the forward's n_contrib) instead of re-testing boxes and transmittances.
+// become gradients once per staged splat, then 3 vector atomics per splat.  With View::contrib_* the forward writes, per
+// tile, the compacted list of the entries some sub-tile composited (with those sub-tiles and the list index), and the
+// backward (REC) stages only that list and walks exactly those pairs, stopping every pixel after its last contributor (the
+// forward's n_contrib) instead of re-testing boxes and transmittances.
 #include "lgr_common.cuh"
 #include "lgr_prof.cuh"
 
@@ -129,21 +130,31 @@ __device__ __forceinline__ void mma_tf32(float& d0, float& d1, float& d2, float&
 // Staged splat: three consecutive float4 per list entry (48-byte stride: conflict-free for 128-bit accesses),
 //   [0] = (px, py, conic_x', conic_y')   [1] = (conic_z', opacity, hx, hy)   [2] = (r, g, b, id as int bits)
 // plus one byte of sub-tile hit bits.
-// recorded: the entry's byte of View::contrib (backward, when the forward recorded which sub-tiles composited it) or nullptr
+// recorded: the entry's word of View::contrib_entry (backward, when the forward recorded which sub-tiles composited it) or
+// nullptr; its sub-tile byte replaces the box test, and its list index replaces hx, which only the box test reads.
 __device__ __forceinline__ void stage_splat(float4* s_rec, unsigned char* s_bits, int slot, const float* __restrict__ splat,
-                                            int id, float tx0, float ty0, const uint8_t* __restrict__ recorded = nullptr) {
+                                            int id, float tx0, float ty0, const uint32_t* __restrict__ recorded = nullptr) {
   const float* rec = splat + (int64_t)id * LGR_SPLAT_FLOATS;
-  const float4 r0 = ldg4(rec), r1 = ldg4(rec + 4);
-  float4 r2 = ldg4(rec + 8);
+  const float4 r0 = ldg4(rec);
+  float4 r1 = ldg4(rec + 4), r2 = ldg4(rec + 8);
   r2.w = __int_as_float(id);
+  unsigned bits;
+  if (recorded) {
+    const uint32_t e = *recorded;
+    bits = e & 0xffu;
+    r1.z = __uint_as_float(e >> 8);
+  } else {
+    bits = subtile_bits(r0, r1, tx0, ty0);
+  }
   s_rec[3 * slot] = r0; s_rec[3 * slot + 1] = r1; s_rec[3 * slot + 2] = r2;
-  s_bits[slot] = recorded ? *recorded : (unsigned char)subtile_bits(r0, r1, tx0, ty0);
+  s_bits[slot] = (unsigned char)bits;
 }
 
 // ---------------------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------------------
-// REC: also record, per tile-list entry, the sub-tiles that composited it (View::contrib), for the backward
+// REC: also write, for the backward, the tile's compacted list of the entries that some sub-tile composited
+// (View::contrib_id / contrib_entry / contrib_count)
 template <bool AUX, bool REC>
 __global__ void __launch_bounds__(BLEND_THREADS, LGR_FWD_MIN_CTAS)
 blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* __restrict__ sorted_ids,
@@ -171,6 +182,7 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   // tid), so the flush of batch b and the staging of batch b+1 need no barrier between them:
   //     stage(0) | A | walk(0) | B | flush(0), stage(1) | A | walk(1) | B | ...
   int base = 0, cnt = min(BATCH, len);
+  int n_rec = 0;                             // REC: entries of the compacted list written so far (the same in every thread)
   auto stage = [&]() {
     if (tid < cnt) stage_splat(s_rec, s_bits, tid, splat, id_next, tx0, ty0);
     else s_bits[tid] = 0;
@@ -250,17 +262,40 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
     }
     const int all_done = __syncthreads_and(done);      // B: every warp has left the walk
     if (AUX && tid < cnt && s_w[tid]) atomicMax(point_weight_bits + __float_as_int(s_rec[3 * tid + 2].w), s_w[tid]);
-    if (REC && tid < cnt) {      // for the backward: which sub-tiles composited this list entry
-      unsigned byte = 0u;
+    if (REC) {
+      // For the backward: the entries of this batch that some sub-tile composited, appended to the tile's compacted list in
+      // list order.  Lane c < 8 of every warp ORs the eight warps' words of chunk c (= staged entries 32c..32c+31, which
+      // warp c's threads own); a scan over lanes 0..7 gives each chunk's offset.
+      unsigned m = 0u;
+      if (lane < BATCH / 32) {
 #pragma unroll
-      for (int w = 0; w < BLEND_THREADS / 32; w++) byte |= ((s_cb[w * (BATCH / 32) + (tid >> 5)] >> (tid & 31)) & 1u) << w;
-      v.contrib[beg + base + tid] = (uint8_t)byte;
+        for (int w = 0; w < BLEND_THREADS / 32; w++) m |= s_cb[w * (BATCH / 32) + lane];
+      }
+      const int c = __popc(m);
+      int incl = c;
+#pragma unroll
+      for (int d = 1; d < BATCH / 32; d <<= 1) {
+        const int y = __shfl_up_sync(FULL, incl, d);
+        if (lane >= d) incl += y;
+      }
+      const unsigned mine = __shfl_sync(FULL, m, warp);
+      const int before = __shfl_sync(FULL, incl - c, warp);
+      if ((mine >> lane) & 1u) {
+        unsigned byte = 0u;
+#pragma unroll
+        for (int w = 0; w < BLEND_THREADS / 32; w++) byte |= ((s_cb[w * (BATCH / 32) + warp] >> lane) & 1u) << w;
+        const int k = beg + n_rec + before + __popc(mine & ((1u << lane) - 1u));
+        v.contrib_id[k] = __float_as_int(s_rec[3 * tid + 2].w);
+        v.contrib_entry[k] = byte | ((uint32_t)(base + tid) << 8);
+      }
+      n_rec += __shfl_sync(FULL, incl, BATCH / 32 - 1);
     }
     base += BATCH;
     if (all_done || base >= len) break;
     cnt = min(BATCH, len - base);
     stage();
   }
+  if (REC && tid == 0) v.contrib_count[tile] = n_rec;
   if (st.inside) {
     const int64_t pix = (int64_t)st.y * v.W + st.x, HW = (int64_t)v.H * v.W;
     image[pix] = C0 + T * __ldg(v.bg);
@@ -301,9 +336,10 @@ constexpr int HITS = 8;          // hits per contraction (half the m of mma.m16n
 constexpr int XROW = 36;         // floats per published row: 32 pixels + 4 pad, so the 8 rows of an ldmatrix block hit 8 bank groups
 constexpr int BWD_SMEM = BATCH * 48 + BATCH * 36 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 192 + 192) * 4 + BATCH;
 
-// REC: the forward recorded (View::contrib) which sub-tiles composited each list entry and (View::last_contrib = its
-// n_contrib output) where every pixel's last contributor sits; the sweep then meets exactly the contributing (sub-tile,
-// splat) pairs and a pixel is finished once the walk has passed its last contributor -- no box tests, no T < 1e-4 test.
+// REC: the forward wrote the compacted list of the entries that some sub-tile composited, with those sub-tiles and the
+// entry's list index (View::contrib_*), and (View::last_contrib = its n_contrib output) where every pixel's last
+// contributor sits; the sweep stages only that list, meets exactly the contributing (sub-tile, splat) pairs, and a pixel
+// is finished once the walk has passed its last contributor -- no box tests, no T < 1e-4 test.
 template <bool REC>
 __global__ void __launch_bounds__(BLEND_THREADS, LGR_BWD_MIN_CTAS)
 blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* __restrict__ sorted_ids,
@@ -339,51 +375,58 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
     Rd = image[pix] * dp0 + image[HW + pix] * dp1 + image[2 * HW + pix] * dp2;
     if (REC) last = v.last_contrib[pix];
   }
-  // B fragments of the moment weights, per warp in shared memory: s_mw[((g*4 + t)*4 + s)*2 + {0,1}] = weight of output g at
-  // the pixel of k-step s with k = t (column t, row s of the sub-tile) / k = t + 4 (column t + 4).  |values| <= 56.25 in
-  // steps of 0.25: exact in TF32.
-  const uint32_t mw_addr = pin_reg(smem_u32(s_mw) + (uint32_t)warp * (192 * 4) + (uint32_t)((min(g, 5) * 4 + t) * 32));
+  // B fragments of the moment weights, per warp in shared memory, lane-major per k-step s (the reading lane l = g*4 + t < 24
+  // takes consecutive 8 bytes, so one LDS.64 of the warp is the minimum two wavefronts):
+  // s_mw[(s*24 + g*4 + t)*2 + {0,1}] = weight of output g at the pixel of k-step s with k = t (column t, row s of the
+  // sub-tile) / k = t + 4 (column t + 4).  |values| <= 56.25 in steps of 0.25: exact in TF32.
+  const uint32_t mw_addr = pin_reg(smem_u32(s_mw) + (uint32_t)warp * (192 * 4) + (uint32_t)((min(g, 5) * 4 + t) * 8));
   for (int k = lane; k < 192; k += 32) {
-    const int which = k & 1, s_ = (k >> 1) & 3, t_ = (k >> 3) & 3, g_ = k >> 5;
+    const int which = k & 1, l_ = (k >> 1) % 24, s_ = (k >> 1) / 24, t_ = l_ & 3, g_ = l_ >> 2;
     const float u = (float)((warp & 1) * 8 + t_ + 4 * which) - 7.5f, vv = (float)((warp >> 1) * 4 + s_) - 7.5f;
     const float f = g_ == 0 ? 1.f : g_ == 1 ? u : g_ == 2 ? vv : g_ == 3 ? u * u : g_ == 4 ? u * vv : vv * vv;
     s_mw[warp * 192 + k] = f;
   }
-  // B fragments of the cotangent weights (columns 0..2 = channel): s_cw[((c*4 + t)*4 + s)*4 + {0,1,2,3}] = hi(k=t), hi(k=t+4), lo(k=t), lo(k=t+4)
-  const uint32_t cw_addr = pin_reg(smem_u32(s_cw) + (uint32_t)warp * (192 * 4) + (uint32_t)((min(g, 2) * 4 + t) * 64));
+  // B fragments of the cotangent weights (columns 0..2 = channel), lane-major per k-step s as above (LDS.128, lanes < 12):
+  // s_cw[(s*12 + c*4 + t)*4 + {0,1,2,3}] = hi(k=t), hi(k=t+4), lo(k=t), lo(k=t+4)
+  const uint32_t cw_addr = pin_reg(smem_u32(s_cw) + (uint32_t)warp * (192 * 4) + (uint32_t)((min(g, 2) * 4 + t) * 16));
   {
     float* cw = s_cw + warp * 192;
     const int col = lane & 7, s = lane >> 3, tt = col & 3, which = col >> 2;
     const float dpc[3] = {dp0, dp1, dp2};
 #pragma unroll
     for (int c = 0; c < 3; c++) {
-      cw[((c * 4 + tt) * 4 + s) * 4 + which] = dpc[c];                  // read as trunc(x) by the tensor core
-      cw[((c * 4 + tt) * 4 + s) * 4 + 2 + which] = tf32_lo(dpc[c]);
+      cw[(s * 12 + c * 4 + tt) * 4 + which] = dpc[c];                   // read as trunc(x) by the tensor core
+      cw[(s * 12 + c * 4 + tt) * 4 + 2 + which] = tf32_lo(dpc[c]);
     }
   }
   __syncwarp();
 
   float T = 1.0f;
   int done = st.inside ? (REC ? (last == 0) : 0) : 1;
-  int id_next = tid < len ? sorted_ids[beg + tid] : -1;
+  // the staged list: REC the forward's compacted list of the tile (n entries), else the whole tile list
+  const int n = REC ? v.contrib_count[tile] : len;
+  const int32_t* __restrict__ ids = REC ? v.contrib_id : sorted_ids;
+  // guarded by len (>= n, in bounds) rather than n, so that the first id load need not wait for the count
+  int id_next = tid < len ? ids[beg + tid] : -1;
+  if (tid >= n) id_next = -1;
 
   // Two barriers per batch, as in the forward: thread tid stages, flushes and re-stages only slot tid (record, hit bits and
   // the nine accumulators of that splat).
-  int base = 0, cnt = min(BATCH, len);
+  int base = 0, cnt = min(BATCH, n);
   auto stage = [&]() {
     if (tid < cnt) {
-      // with View::contrib: walk exactly the (sub-tile, splat) pairs that composited something in the forward
-      stage_splat(s_rec, s_bits, tid, splat, id_next, tx0, ty0, REC ? v.contrib + beg + base + tid : nullptr);
+      // REC: walk exactly the (sub-tile, splat) pairs that composited something in the forward
+      stage_splat(s_rec, s_bits, tid, splat, id_next, tx0, ty0, REC ? v.contrib_entry + beg + base + tid : nullptr);
 #pragma unroll
       for (int k = 0; k < 9; k++) s_g[tid * 9 + k] = 0.f;
     } else {
       s_bits[tid] = 0;
     }
-    id_next = base + BATCH + tid < len ? sorted_ids[beg + base + BATCH + tid] : -1;
+    id_next = base + BATCH + tid < n ? ids[beg + base + BATCH + tid] : -1;
     if (id_next >= 0) prefetch_l2(splat + (int64_t)id_next * LGR_SPLAT_FLOATS);
   };
-  if (len > 0) stage();
-  while (base < len) {
+  if (n > 0) stage();
+  while (base < n) {
     __syncthreads();                         // A: the batch is staged
     if (!__all_sync(FULL, done)) {
       int c0 = -32, pend = 0, my_e = 0;
@@ -422,13 +465,15 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
           if (REC) {
             // every visited splat in front of the pixel's last contributor with alpha >= 1/255 was composited by the forward
             // (it would otherwise have stopped the pixel there); same multiplications, so T follows the forward bit for bit
+            // (the staged record holds the entry's index in the tile list where the box test's hx was)
+            const int iA = __float_as_int(s_rec[3 * eA + 1].z), iB = __float_as_int(s_rec[3 * eB + 1].z);
             cA = !done && powerA <= 0.0f && alphaA >= ALPHA_MIN;
             if (cA) T = __fmul_rn(T, omA);
-            done = (base + eA + 1 >= last);
+            done = (iA + 1 >= last);
             TB = T;
             cB = two && !done && powerB <= 0.0f && alphaB >= ALPHA_MIN;
             if (cB) T = __fmul_rn(T, omB);
-            if (two) done = (base + eB + 1 >= last);
+            if (two) done = (iB + 1 >= last);
           } else {
             if (!done && powerA <= 0.0f && alphaA >= ALPHA_MIN) {
               const float tt = __fmul_rn(T, omA);
@@ -487,8 +532,8 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
             const uint32_t l2 = __float_as_uint(tf32_lo(__uint_as_float(a2))), l3 = __float_as_uint(tf32_lo(__uint_as_float(a3)));
             float2 bm = make_float2(0.f, 0.f);
             float4 bc = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (g < 6) bm = lds_f2(mw_addr + 8u * s);
-            if (g < 3) bc = lds_f4(cw_addr + 16u * s);
+            if (g < 6) bm = lds_f2(mw_addr + 192u * s);
+            if (g < 3) bc = lds_f4(cw_addr + 192u * s);
             mma_tf32(d0, d1, z0, z1, a0, a1, a2, a3, __float_as_uint(bm.x), __float_as_uint(bm.y));
             mma_tf32(y0, y1, d2, d3, a0, a1, a2, a3, __float_as_uint(bc.x), __float_as_uint(bc.y));
             mma_tf32(d0, d1, z0, z1, l0, l1, l2, l3, __float_as_uint(bm.x), __float_as_uint(bm.y));
@@ -538,8 +583,8 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
       }
     }
     base += BATCH;
-    if (all_done || base >= len) break;
-    cnt = min(BATCH, len - base);
+    if (all_done || base >= n) break;
+    cnt = min(BATCH, n - base);
     stage();
   }
 }
@@ -552,7 +597,7 @@ int launch_blend_fwd(const View& v, const int32_t* tile_start, const int32_t* so
   if (ntiles <= 0) return 0;
   ProfScope ps(K_BLEND_FWD, st);
   unsigned* pwb = reinterpret_cast<unsigned*>(point_weight);
-  const bool rec = v.contrib != nullptr;
+  const bool rec = v.contrib_id != nullptr && v.contrib_entry != nullptr && v.contrib_count != nullptr;
   if (v.want_aux && rec)
     blend_fwd_kernel<true, true><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
   else if (v.want_aux)
@@ -570,7 +615,7 @@ int launch_blend_bwd(const View& v, const int32_t* tile_start, const int32_t* so
   const int ntiles = v.gx * (v.row1 - v.row0);
   if (ntiles <= 0) return 0;
   // > 48 KB of dynamic shared memory needs the opt-in; the attribute is per device and cheap to set, so set it every time
-  const bool rec = v.contrib != nullptr && v.last_contrib != nullptr;
+  const bool rec = v.contrib_id != nullptr && v.contrib_entry != nullptr && v.contrib_count != nullptr && v.last_contrib != nullptr;
   cudaError_t e = rec ? cudaFuncSetAttribute(blend_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM)
                       : cudaFuncSetAttribute(blend_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
   if (e != cudaSuccess) return (int)e;

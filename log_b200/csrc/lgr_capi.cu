@@ -51,6 +51,8 @@ static bool view_ok(const lgr_view* v) {
   if (v->region_count_d && (v->num_regions <= 0 || v->num_regions > LGR_SHARD_MAX_RANKS || v->region_cap <= 0 || v->num_owners > 0 ||
                             v->gather_index_d))
     return false;
+  const int lists = (v->contrib_id_d != nullptr) + (v->contrib_entry_d != nullptr) + (v->contrib_count_d != nullptr);
+  if (lists != 0 && lists != 3) return false;      // the compacted contribution list comes whole or not at all
   return true;
 }
 
@@ -129,6 +131,7 @@ int lgr_forward_render(const lgr_view* view, int64_t n, int64_t num_instances, i
   if (num_instances > 0 && (!inst_key_d || !inst_val_d || !sorted_ids_d || !splat_d || !radii_d)) return LGR_E_BADARG;
   if (view->want_aux && (!point_id_pixel_d || !point_weight_pixel_d || (n > 0 && !point_weight_d))) return LGR_E_BADARG;
   if (num_instances > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  if (view->contrib_id_d && max_tile_len > LGR_CONTRIB_MAX_LIST) return LGR_E_UNSUPPORTED;      // list indices would not fit
   cudaStream_t st = (cudaStream_t)stream;
   const View v = make_view(view, n);
   int rc = launch_bin_and_sort(v, n, num_instances, max_tile_len, num_long_tiles, splat_d, radii_d, const_cast<int32_t*>(tile_start_d), tile_cursor_d,
@@ -150,6 +153,8 @@ int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t ins
   if (n > 0 && (!splat_d || !radii_d)) return LGR_E_BADARG;
   if (view->want_aux && (!point_id_pixel_d || !point_weight_pixel_d || (n > 0 && !point_weight_d))) return LGR_E_BADARG;
   if (instance_capacity > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  // contrib_entry_d's list indices: a list longer than lgr_sort_smem_capacity() (far below LGR_CONTRIB_MAX_LIST) already
+  // raises meta_d[6] bit 1, so no valid output of this call depends on an index that did not fit
   cudaStream_t st = (cudaStream_t)stream;
   const View v = make_view(view, n);
   int rc = launch_bin_and_sort(v, n, instance_capacity, 0, 0, splat_d, radii_d, tile_start_d, tile_cursor_d, inst_key_d, inst_val_d,

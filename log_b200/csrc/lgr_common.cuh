@@ -35,7 +35,11 @@ struct View {
   int32_t* tile_rank;        // (rows,4) or NULL: slots of the <= 4 tiles of a small splat, taken by the counting pass
   const int64_t* gather;     // (n) or NULL: input row of output row i (gather fused into the projection, SURVEY 8(f) row 3)
   const int32_t* pid_map;    // (n) or NULL: point_id_pixel = pid_map[winning row]
-  uint8_t* contrib;          // (instances) or NULL: per list entry, the sub-tiles with a contributing pixel (forward -> backward)
+  // (instances) or NULL, forward -> backward: per tile, the list entries some pixel composited, compacted in list order at
+  // tile_start[t]: the id, and (sub-tiles that composited it | list index << 8); contrib_count[t] = how many
+  int32_t* contrib_id;
+  uint32_t* contrib_entry;
+  int32_t* contrib_count;    // (tiles)
   const int32_t* last_contrib;   // (H,W) or NULL: the forward's n_contrib (list index + 1 of each pixel's last contributor), backward only
   const int32_t* region_count;   // (regions) or NULL: rows = regions x region_cap, the first region_count[s] rows of region s in use
   int64_t region_cap;
@@ -51,7 +55,7 @@ struct View {
 
 inline View make_view(const lgr_view* v, int64_t n = 0) {
   View o;
-  o.num_owners = v->num_owners; o.band_ids = v->band_ids_d; o.band_blk = v->band_blk_d; o.band_count = v->band_count_d; o.band_rows = v->band_rows_d; o.band_dsplat = v->band_dsplat_d; o.tile_rank = v->tile_rank_d; o.gather = v->gather_index_d; o.pid_map = v->pid_map_d; o.contrib = v->contrib_d; o.last_contrib = v->last_contrib_d;
+  o.num_owners = v->num_owners; o.band_ids = v->band_ids_d; o.band_blk = v->band_blk_d; o.band_count = v->band_count_d; o.band_rows = v->band_rows_d; o.band_dsplat = v->band_dsplat_d; o.tile_rank = v->tile_rank_d; o.gather = v->gather_index_d; o.pid_map = v->pid_map_d; o.contrib_id = v->contrib_id_d; o.contrib_entry = v->contrib_entry_d; o.contrib_count = v->contrib_count_d; o.last_contrib = v->last_contrib_d;
   o.region_count = v->region_count_d; o.region_cap = v->region_cap; o.regions = v->region_count_d ? v->num_regions : 0;
   o.cov3d = v->cov3D_precomp_d; o.dcov3d = v->dcov3D_d;
   o.owner_chunk = o.num_owners > 0 ? (int)LGR_OWNER_CHUNK(n, (int64_t)o.num_owners) : 256;

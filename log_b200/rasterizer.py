@@ -29,7 +29,7 @@ from ._capi import LGR_FILTER_ADD, LGR_FILTER_MAX, LGR_FILTER_NONE, LgrView
 PREZERO_DSPLAT = bool(int(__import__('os').environ.get('LGR_PREZERO_DSPLAT', '0')))      # see rasterize_forward
 # tile slots taken once, by the counting pass (lgr_view.tile_rank_d); 0 = the two-pass binning of round 1 (A/B knob)
 RANKED_BIN = bool(int(__import__('os').environ.get('LGR_RANKED_BIN', '1')))
-# the forward blend records, per tile-list entry, the sub-tiles that composited it; the backward walks only those (A/B knob)
+# the forward blend lists the entries some pixel composited, with their sub-tiles; the backward stages and walks only those (A/B knob)
 CONTRIB_BITS = bool(int(__import__('os').environ.get('LGR_CONTRIB_BITS', '1')))
 FLAVOUR_STOCK = 'stock'   # diff_gaussian_rasterization            (graphdeco-inria)   -> 2-tuple, cov += 0.3
 FLAVOUR_FORK = 'fork'     # diff_gaussian_rasterization_wodilate   (chingswy antialias) -> 5-tuple, cov = max(cov, 0.3)
@@ -105,6 +105,24 @@ def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: boo
     v.campos_d = cp.data_ptr() if cp is not None else None
     v.bg_d = bg.data_ptr()
     return v
+
+
+def set_contrib_lists(view, buf, D, n_contrib):
+    """Point `view` at the forward -> backward contribution lists (lgr_view.contrib_id_d / contrib_entry_d /
+    contrib_count_d), held in `buf` -- int32, >= 2 D + tiles: D ids, D entries, one count per tile -- and at the forward's
+    n_contrib (last_contrib_d); buf None: neither (the backward re-tests boxes and transmittances)."""
+    if buf is None:
+        view.contrib_id_d = view.contrib_entry_d = view.contrib_count_d = view.last_contrib_d = None
+        return
+    p = buf.data_ptr()
+    view.contrib_id_d, view.contrib_entry_d, view.contrib_count_d = p, p + 4 * D, p + 8 * D
+    view.last_contrib_d = n_contrib.data_ptr()
+
+
+def use_contrib_lists(D, max_tile_len):
+    """Record the contribution lists for the backward?  (Not for an empty view, nor for a tile list longer than the entry
+    word's index field; max_tile_len None: a device-sized call, whose lists are bounded by lgr_sort_smem_capacity().)"""
+    return CONTRIB_BITS and D > 0 and (max_tile_len is None or max_tile_len <= _capi.LGR_CONTRIB_MAX_LIST)
 
 
 class RasterState:
@@ -206,10 +224,9 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         D, max_len, num_long, stock_D, m = int(instance_capacity), None, None, None, None
         inst_key, inst_val = torch.empty((D,), **u32), torch.empty((D,), **u32)
         sorted_ids = torch.empty((D,), **i32)
-        contrib = torch.empty((D,), dtype=torch.uint8, device=dev) if CONTRIB_BITS else None
+        contrib = torch.empty((2 * D + ntiles,), **i32) if use_contrib_lists(D, None) else None
         keep.append(contrib)
-        view.contrib_d = contrib.data_ptr() if contrib is not None and D > 0 else None
-        view.last_contrib_d = n_contrib.data_ptr() if view.contrib_d else None
+        set_contrib_lists(view, contrib, D, n_contrib)
         _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(view), n, D, _ptr(meta), _ptr(splat), _ptr(radii), _ptr(tile_start),
                                                         _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(sorted_ids), _ptr(image),
                                                         _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp), _ptr(pw), _ptr(pc), st),
@@ -225,10 +242,11 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         inst_val = torch.empty((D,), **u32)
         inst_tmp = torch.empty((2 * D,), **u32) if max_len > lib.lgr_sort_smem_capacity() else None
         sorted_ids = torch.empty((D,), **i32)
-        contrib = torch.empty((D,), dtype=torch.uint8, device=dev) if CONTRIB_BITS else None      # forward -> backward: see lgr_view.contrib_d
+        # forward -> backward: the entries some pixel composited (lgr_view.contrib_*); the backward stages only those and
+        # stops a pixel after its last contributor
+        contrib = torch.empty((2 * D + ntiles,), **i32) if use_contrib_lists(D, max_len) else None
         keep.append(contrib)
-        view.contrib_d = contrib.data_ptr() if contrib is not None and D > 0 else None
-        view.last_contrib_d = n_contrib.data_ptr() if view.contrib_d else None      # the backward stops a pixel after its last contributor
+        set_contrib_lists(view, contrib, D, n_contrib)
         _capi.check(lib.lgr_forward_render(ctypes.byref(view), n, D, max_len, num_long, _ptr(splat), _ptr(radii), _ptr(tile_start),
                                            _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp),
                                            _ptr(sorted_ids), _ptr(image), _ptr(final_T), _ptr(n_contrib), _ptr(pid),

@@ -319,7 +319,7 @@ class SplatExchange:
         point_id_pixel with GLOBAL Gaussian indices, point_weight_pixel); image / maps are full size, band rows filled."""
         import ctypes
         from . import _capi
-        from .rasterizer import CONTRIB_BITS, _ptr, _stream
+        from .rasterizer import _ptr, _stream, set_contrib_lists, use_contrib_lists
         lib = _capi.load()
         dev = self.buf.device
         v = s.view_band
@@ -351,8 +351,8 @@ class SplatExchange:
             inst_key = self._scratch('inst_key', (cap,), torch.int32)
             inst_val = self._scratch('inst_val', (cap,), torch.int32)
             s.sorted_ids = self._scratch('sorted_ids', (cap,), torch.int32)
-            v.contrib_d = self._scratch('contrib', (cap,), torch.uint8).data_ptr() if CONTRIB_BITS else None
-            v.last_contrib_d = n_contrib.data_ptr() if v.contrib_d else None
+            set_contrib_lists(v, self._scratch('contrib', (2 * cap + ntiles,), torch.int32) if use_contrib_lists(cap, None) else None,
+                              cap, n_contrib)
             s.num_instances, s.max_tile_len, s.num_rows, s.stock_instances = cap, None, None, None      # see stats()
             _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(v), rows, cap, _ptr(meta), _ptr(self.recv_splat), _ptr(self.recv_radii),
                                                             _ptr(s.tile_start), _ptr(cursor), _ptr(inst_key), _ptr(inst_val), _ptr(s.sorted_ids),
@@ -370,8 +370,8 @@ class SplatExchange:
         inst_val = self._scratch('inst_val', (D,), torch.int32)
         inst_tmp = self._scratch('inst_tmp', (2 * D,), torch.int32) if max_len > lib.lgr_sort_smem_capacity() else None
         s.sorted_ids = self._scratch('sorted_ids', (D,), torch.int32)
-        v.contrib_d = self._scratch('contrib', (D,), torch.uint8).data_ptr() if CONTRIB_BITS and D > 0 else None
-        v.last_contrib_d = n_contrib.data_ptr() if v.contrib_d else None
+        set_contrib_lists(v, self._scratch('contrib', (2 * D + ntiles,), torch.int32) if use_contrib_lists(D, max_len) else None,
+                          D, n_contrib)
         _capi.check(lib.lgr_forward_render(ctypes.byref(v), rows, D, max_len, num_long, _ptr(self.recv_splat), _ptr(self.recv_radii),
                                            _ptr(s.tile_start), _ptr(cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp),
                                            _ptr(s.sorted_ids), _ptr(s.image), _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp),
