@@ -129,7 +129,7 @@ class RasterState:
     """Buffers produced by the forward and consumed by the backward (kept alive by autograd)."""
     __slots__ = ('view', 'keep', 'n', 'num_instances', 'max_tile_len', 'stock_instances', 'num_visible', 'splat',
                  'radii', 'clamped', 'tile_start', 'sorted_ids', 'final_T', 'n_contrib', 'image', 'sh', 'num_owners',
-                 'band_ids', 'band_count', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D')
+                 'band_ids', 'band_count', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D', 'contrib')
 
     def read_stats(self):
         """Counters of this forward, read back from meta_d (synchronises): D, longest tile list, D by the stock rule, visible
@@ -137,6 +137,15 @@ class RasterState:
         m = self.meta.tolist()
         return dict(num_instances=int(m[0]), max_tile_len=int(m[1]), stock_instances=(m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32),
                     num_visible=int(m[4]), overflow=int(m[6]))
+
+    def contrib_lists(self):
+        """The compacted contribution lists the forward wrote for the backward (lgr_view.contrib_*), as int32 views:
+        (ids, entry words = sub-tile byte | list index << 8, per-tile counts); None when the forward recorded none.  Tile t's
+        entries start at tile_start[t]."""
+        if self.contrib is None:
+            return None
+        D = self.num_instances
+        return self.contrib[:D], self.contrib[D:2 * D], self.contrib[2 * D:]
 
 
 def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_precomp, shs, filter_mode, want_aux,
@@ -259,6 +268,7 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     s.splat, s.radii, s.clamped, s.tile_start, s.sorted_ids = splat, radii, clamped, tile_start, sorted_ids
     s.final_T, s.n_contrib, s.image, s.sh = final_T, n_contrib, image, shs is not None
     s.point_count = pc
+    s.contrib = contrib
     s.num_owners, s.band_ids, s.band_count = num_owners, (band_ids, band_blk, band_rows, band_dsplat), band_count
     s.band_counts_host = [int(x) for x in m[_capi.LGR_META_INTS:]] if num_owners > 0 else None
     return image, radii, pid, pwp, pw, s
