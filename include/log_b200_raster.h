@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 17
+#define LGR_ABI_VERSION 18
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -108,7 +108,15 @@ typedef struct lgr_view {
                             follows the rows a rank received, not the size of the exchange buffer. */
   int64_t region_cap;    /* rows per region (with region_count_d) */
   int32_t num_regions;   /* 1 .. LGR_SHARD_MAX_RANKS (with region_count_d) */
-  int32_t reserved0;
+  int32_t num_channels;  /* precomputed colour channels: 0 or 3 = three (r, g, b); 6 = six, composited in one pass with the
+                            same transmittances (e.g. colour and LoG's (depth, height, 1) pass).  With 6: colors_precomp_d is
+                            (N,6), image_d, dL_dimage_d (6,H,W), bg_d (6,), dcolors_d (N,6), and splat_ext_d is required.
+                            Channels 0..2 equal, bit for bit, a 3-channel call with colours [:, :3] and bg[:3]; channels
+                            3..5 one with [:, 3:] and bg[3:].  Not available with shs_d, raw_params, gather_index_d, band
+                            mode (num_owners > 0) or shard mode (region_count_d, pid_map_d, lgr_shard_*): LGR_E_UNSUPPORTED. */
+  float* splat_ext_d;    /* (N,4) or NULL: with num_channels = 6, the fourth float4 of every projected record, (c3, c4, c5, 0),
+                            written by lgr_forward_project and read by lgr_forward_render[_device_sized] / lgr_backward /
+                            lgr_blend_backward.  The (N,12) splat record (read by the bin and sort kernels) is unchanged. */
   const float* cov3D_precomp_d; /* (N,6) or NULL: the stock API's cov3D_precomp (upper triangle xx xy xz yy yz zz of the world-space
                             covariance, diff_gaussian_rasterization's layout).  When set, lgr_forward_project / lgr_backward
                             take the covariance from here (scale_modifier is NOT applied, as in the stock rasteriser),
@@ -119,7 +127,7 @@ typedef struct lgr_view {
   const float* viewmatrix_d; /* (4,4) world_view_transform, stored transposed (LoG/dataset/base.py:40-46) */
   const float* projmatrix_d; /* (4,4) full_proj_transform, same convention */
   const float* campos_d;     /* (3,) */
-  const float* bg_d;         /* (3,) */
+  const float* bg_d;         /* (3,), or (6,) with num_channels = 6 */
 } lgr_view;
 
 /* Sizes of the buffers the caller must provide. */
@@ -147,6 +155,7 @@ int lgr_mark_visible(int64_t n, const float* means3D_d, const float* viewmatrix_
 
 /* Stage 1 of the forward: per-Gaussian projection + EWA covariance + colour, tile counting, tile scan.
  *   in : means3D (N,3) opacities (N) scales (N,3) rotations (N,4); colors_precomp (N,3) XOR shs (N,K,3)
+ *        (colors_precomp (N,6) with view->num_channels = 6; splat_ext_d then receives (N,4))
  *   out: splat_d (N,12) radii_d (N) int32; clamped_d (N) uint8 (SH only, may be NULL with colors_precomp);
  *        tile_start_d (tiles+1) int32 exclusive scan of per-tile counts (tiles = gx * rows rendered);
  *        tile_cursor_d (LGR_TILE_SCRATCH_INTS*tiles) int32 scratch; meta_d (LGR_META_INTS) int32.
@@ -160,7 +169,7 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
  *   num_instances / max_tile_len / num_long_tiles : the values read from meta_d[0], meta_d[1], meta_d[5]
  *   scratch: inst_key_d, inst_val_d (num_instances) uint32; inst_tmp_d (2*num_instances) uint32, only needed when
  *            max_tile_len exceeds the shared-memory sort capacity (lgr_sort_smem_capacity()), else may be NULL
- *   out: sorted_ids_d (num_instances) int32 (kept for backward); image_d (3,H,W); final_T_d (H,W);
+ *   out: sorted_ids_d (num_instances) int32 (kept for backward); image_d (3,H,W) (6,H,W with num_channels = 6); final_T_d (H,W);
  *        n_contrib_d (H,W) int32; when view->want_aux: point_id_pixel_d (H,W) int32, point_weight_pixel_d (H,W),
  *        point_weight_d (N) -- must be zero-filled by the caller;
  *        point_count_d (N) int32 or NULL -- zero-filled by the caller; receives, per Gaussian, the number of pixels whose
@@ -192,7 +201,8 @@ int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t ins
  * behind each splat), then per-Gaussian projection backward.
  *   image_d (3,H,W): the forward's output, unmodified.  dsplat_d (N,12) scratch, zero-filled by the caller.
  *   out (each written for every Gaussian; culled ones get 0): dmeans3D (N,3) dmeans2D (N,3; d/d(ndc x,y), z = 0)
- *        dopacities (N) dscales (N,3) drotations (N,4) and dcolors (N,3) XOR dshs (N,K,3). */
+ *        dopacities (N) dscales (N,3) drotations (N,4) and dcolors (N,3) XOR dshs (N,K,3).
+ *   With view->num_channels = 6: image_d / dL_dimage_d (6,H,W), dcolors_d (N,6); dsplat_d floats 9..11 carry d/dc3..5. */
 int lgr_backward(const lgr_view* view, int64_t n, int64_t num_instances, const float* means3D_d,
                  const float* opacities_d, const float* scales_d, const float* rotations_d,
                  const float* colors_precomp_d, const float* shs_d, const float* splat_d, const int32_t* radii_d,

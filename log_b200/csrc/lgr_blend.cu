@@ -26,6 +26,14 @@ constexpr int BLEND_THREADS = TILE_PIX;   // 256
 #ifndef LGR_BWD_MIN_CTAS
 #define LGR_BWD_MIN_CTAS 4
 #endif
+// the six-channel instantiations (View::num_channels = 6): three more accumulators in the forward; in the backward ~64 KB of
+// shared memory per CTA, which leaves room for 3 CTAs per SM
+#ifndef LGR_FWD6_MIN_CTAS
+#define LGR_FWD6_MIN_CTAS 4
+#endif
+#ifndef LGR_BWD6_MIN_CTAS
+#define LGR_BWD6_MIN_CTAS 3
+#endif
 constexpr int BATCH = 256;
 constexpr unsigned FULL = 0xffffffffu;
 
@@ -129,14 +137,20 @@ __device__ __forceinline__ void mma_tf32(float& d0, float& d1, float& d2, float&
 
 // Staged splat: three consecutive float4 per list entry (48-byte stride: conflict-free for 128-bit accesses),
 //   [0] = (px, py, conic_x', conic_y')   [1] = (conic_z', opacity, hx, hy)   [2] = (r, g, b, id as int bits)
-// plus one byte of sub-tile hit bits.
+// plus one byte of sub-tile hit bits.  SIX (six colour channels): a fourth float4 [3] = (c3, c4, c5, 0) from View::splat_ext
+// (64-byte stride, also conflict-free).
 // recorded: the entry's word of View::contrib_entry (backward, when the forward recorded which sub-tiles composited it) or
 // nullptr; its sub-tile byte replaces the box test, and its list index replaces hx, which only the box test reads.
+template <bool SIX = false>
 __device__ __forceinline__ void stage_splat(float4* s_rec, unsigned char* s_bits, int slot, const float* __restrict__ splat,
-                                            int id, float tx0, float ty0, const uint32_t* __restrict__ recorded = nullptr) {
+                                            int id, float tx0, float ty0, const uint32_t* __restrict__ recorded = nullptr,
+                                            const float* __restrict__ splat_ext = nullptr) {
+  constexpr int F4 = SIX ? 4 : 3;
   const float* rec = splat + (int64_t)id * LGR_SPLAT_FLOATS;
   const float4 r0 = ldg4(rec);
   float4 r1 = ldg4(rec + 4), r2 = ldg4(rec + 8);
+  float4 r3;
+  if (SIX) r3 = ldg4(splat_ext + 4 * (int64_t)id);
   r2.w = __int_as_float(id);
   unsigned bits;
   if (recorded) {
@@ -146,7 +160,8 @@ __device__ __forceinline__ void stage_splat(float4* s_rec, unsigned char* s_bits
   } else {
     bits = subtile_bits(r0, r1, tx0, ty0);
   }
-  s_rec[3 * slot] = r0; s_rec[3 * slot + 1] = r1; s_rec[3 * slot + 2] = r2;
+  s_rec[F4 * slot] = r0; s_rec[F4 * slot + 1] = r1; s_rec[F4 * slot + 2] = r2;
+  if (SIX) s_rec[F4 * slot + 3] = r3;
   s_bits[slot] = (unsigned char)bits;
 }
 
@@ -155,13 +170,18 @@ __device__ __forceinline__ void stage_splat(float4* s_rec, unsigned char* s_bits
 // ---------------------------------------------------------------------------------------------------------
 // REC: also write, for the backward, the tile's compacted list of the entries that some sub-tile composited
 // (View::contrib_id / contrib_entry / contrib_count)
-template <bool AUX, bool REC>
-__global__ void __launch_bounds__(BLEND_THREADS, LGR_FWD_MIN_CTAS)
+// SIX: composite six colour channels (View::num_channels = 6).  Channels 3..5 come from the staged record's fourth float4 and
+// get their own accumulators with the same fmaf per channel, and no decision reads them, so channels 0..2 and 3..5 equal a
+// three-channel render of either half bit for bit.
+template <bool AUX, bool REC, bool SIX = false>
+__global__ void __launch_bounds__(BLEND_THREADS, SIX ? LGR_FWD6_MIN_CTAS : LGR_FWD_MIN_CTAS)
 blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* __restrict__ sorted_ids,
                  const float* __restrict__ splat, float* __restrict__ image, float* __restrict__ final_T,
                  int32_t* __restrict__ n_contrib, int32_t* __restrict__ pid_pixel, float* __restrict__ pw_pixel,
                  unsigned* __restrict__ point_weight_bits, int32_t* __restrict__ point_count) {
-  __shared__ float4 s_rec[BATCH * 3];
+  constexpr int F4 = SIX ? 4 : 3;             // float4 per staged record
+  constexpr uint32_t RB = 16u * F4;            // its stride in bytes
+  __shared__ float4 s_rec[BATCH * F4];
   __shared__ unsigned s_w[AUX ? BATCH : 1];
   __shared__ unsigned char s_bits[BATCH];
   __shared__ unsigned s_cb[REC ? (BLEND_THREADS / 32) * (BATCH / 32) : 1];      // per warp: bit e = a pixel of this warp took staged splat e
@@ -174,6 +194,7 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   const uint32_t s_rec_addr = pin_reg(smem_u32(s_rec));
 
   float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, wmax = 0.f;
+  float C3 = 0.f, C4 = 0.f, C5 = 0.f;          // SIX only
   int last = 0, wid = -1;
   int done = st.inside ? 0 : 1;
   int id_next = tid < len ? sorted_ids[beg + tid] : -1;
@@ -184,11 +205,12 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   int base = 0, cnt = min(BATCH, len);
   int n_rec = 0;                             // REC: entries of the compacted list written so far (the same in every thread)
   auto stage = [&]() {
-    if (tid < cnt) stage_splat(s_rec, s_bits, tid, splat, id_next, tx0, ty0);
+    if (tid < cnt) stage_splat<SIX>(s_rec, s_bits, tid, splat, id_next, tx0, ty0, nullptr, v.splat_ext);
     else s_bits[tid] = 0;
     if (AUX) s_w[tid] = 0u;
     id_next = base + BATCH + tid < len ? sorted_ids[beg + base + BATCH + tid] : -1;
     if (id_next >= 0) prefetch_l2(splat + (int64_t)id_next * LGR_SPLAT_FLOATS);
+    if (SIX && id_next >= 0) prefetch_l2(v.splat_ext + 4 * (int64_t)id_next);
   };
   if (len > 0) stage();
   while (base < len) {
@@ -210,7 +232,7 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
           const bool two = mask != 0u;
           const int jB = two ? __ffs(mask) - 1 : jA;
           mask &= mask - 1;
-          const uint32_t recA = s_rec_addr + 48u * (uint32_t)(c0 + jA), recB = s_rec_addr + 48u * (uint32_t)(c0 + jB);
+          const uint32_t recA = s_rec_addr + RB * (uint32_t)(c0 + jA), recB = s_rec_addr + RB * (uint32_t)(c0 + jB);
           const float4 r0A = lds_f4(recA), r0B = lds_f4(recB);
           const float2 r1A = lds_f2(recA + 16u), r1B = lds_f2(recB + 16u);                  // (conic_z, opacity)
           const float dxA = __fsub_rn(r0A.x, pxf), dyA = __fsub_rn(r0A.y, pyf);
@@ -225,6 +247,10 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
               wA = alphaA * T;
               const float4 r2 = lds_f4(recA + 32u);
               C0 = fmaf(r2.x, wA, C0); C1 = fmaf(r2.y, wA, C1); C2 = fmaf(r2.z, wA, C2);
+              if (SIX) {
+                const float4 r3 = lds_f4(recA + 48u);
+                C3 = fmaf(r3.x, wA, C3); C4 = fmaf(r3.y, wA, C4); C5 = fmaf(r3.z, wA, C5);
+              }
               T = test_T;
               last = base + c0 + jA + 1;
               if (AUX && wA > wmax) { wmax = wA; wid = __float_as_int(r2.w); }
@@ -237,6 +263,10 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
               wB = alphaB * T;
               const float4 r2 = lds_f4(recB + 32u);
               C0 = fmaf(r2.x, wB, C0); C1 = fmaf(r2.y, wB, C1); C2 = fmaf(r2.z, wB, C2);
+              if (SIX) {
+                const float4 r3 = lds_f4(recB + 48u);
+                C3 = fmaf(r3.x, wB, C3); C4 = fmaf(r3.y, wB, C4); C5 = fmaf(r3.z, wB, C5);
+              }
               T = test_T;
               last = base + c0 + jB + 1;
               if (AUX && wB > wmax) { wmax = wB; wid = __float_as_int(r2.w); }
@@ -261,7 +291,7 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
       }
     }
     const int all_done = __syncthreads_and(done);      // B: every warp has left the walk
-    if (AUX && tid < cnt && s_w[tid]) atomicMax(point_weight_bits + __float_as_int(s_rec[3 * tid + 2].w), s_w[tid]);
+    if (AUX && tid < cnt && s_w[tid]) atomicMax(point_weight_bits + __float_as_int(s_rec[F4 * tid + 2].w), s_w[tid]);
     if (REC) {
       // For the backward: the entries of this batch that some sub-tile composited, appended to the tile's compacted list in
       // list order.  Lane c < 8 of every warp ORs the eight warps' words of chunk c (= staged entries 32c..32c+31, which
@@ -285,7 +315,7 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
 #pragma unroll
         for (int w = 0; w < BLEND_THREADS / 32; w++) byte |= ((s_cb[w * (BATCH / 32) + warp] >> lane) & 1u) << w;
         const int k = beg + n_rec + before + __popc(mine & ((1u << lane) - 1u));
-        v.contrib_id[k] = __float_as_int(s_rec[3 * tid + 2].w);
+        v.contrib_id[k] = __float_as_int(s_rec[F4 * tid + 2].w);
         v.contrib_entry[k] = byte | ((uint32_t)(base + tid) << 8);
       }
       n_rec += __shfl_sync(FULL, incl, BATCH / 32 - 1);
@@ -301,6 +331,11 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
     image[pix] = C0 + T * __ldg(v.bg);
     image[HW + pix] = C1 + T * __ldg(v.bg + 1);
     image[2 * HW + pix] = C2 + T * __ldg(v.bg + 2);
+    if (SIX) {
+      image[3 * HW + pix] = C3 + T * __ldg(v.bg + 3);
+      image[4 * HW + pix] = C4 + T * __ldg(v.bg + 4);
+      image[5 * HW + pix] = C5 + T * __ldg(v.bg + 5);
+    }
     final_T[pix] = T;
     n_contrib[pix] = last;
     if (AUX) {
@@ -335,22 +370,31 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
 constexpr int HITS = 8;          // hits per contraction (half the m of mma.m16n8k8: 8 wG rows + 8 w rows)
 constexpr int XROW = 36;         // floats per published row: 32 pixels + 4 pad, so the 8 rows of an ldmatrix block hit 8 bank groups
 constexpr int BWD_SMEM = BATCH * 48 + BATCH * 36 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 192 + 192) * 4 + BATCH;
+// six channels: 64-byte records, 12 accumulators per splat, a cotangent table of 6 columns (65 792 bytes)
+constexpr int BWD6_SMEM = BATCH * 64 + BATCH * 48 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 384 + 192) * 4 + BATCH;
 
 // REC: the forward wrote the compacted list of the entries that some sub-tile composited, with those sub-tiles and the
 // entry's list index (View::contrib_*), and (View::last_contrib = its n_contrib output) where every pixel's last
 // contributor sits; the sweep stages only that list, meets exactly the contributing (sub-tile, splat) pairs, and a pixel
 // is finished once the walk has passed its last contributor -- no box tests, no T < 1e-4 test.
-template <bool REC>
-__global__ void __launch_bounds__(BLEND_THREADS, LGR_BWD_MIN_CTAS)
+// SIX: six colour channels.  R_j and c . dL/dC run over the six; the cotangent B operand fills 6 of the 8 columns (same mma
+// count); 12 accumulators per splat (moments, then the six colour sums), flushed with three float4 atomics.
+template <bool REC, bool SIX = false>
+__global__ void __launch_bounds__(BLEND_THREADS, SIX ? LGR_BWD6_MIN_CTAS : LGR_BWD_MIN_CTAS)
 blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* __restrict__ sorted_ids,
                  const float* __restrict__ splat, const float* __restrict__ image,
                  const float* __restrict__ dL_dimage, float* __restrict__ dsplat) {
+  constexpr int F4 = SIX ? 4 : 3;                // float4 per staged record
+  constexpr uint32_t RB = 16u * F4;             // its stride in bytes
+  constexpr int NCH = SIX ? 6 : 3;              // colour channels = used columns of the cotangent B operand
+  constexpr int NG = 6 + NCH;                   // accumulators per staged splat: 6 moments + the colour sums
+  constexpr int NCW = 64 * NCH;                 // floats of a warp's cotangent table: 4 k-steps x NCH*4 lanes x 4
   extern __shared__ float4 smem_f4[];
-  float4* s_rec = smem_f4;                                                        // [BATCH * 3]
-  float* s_g = reinterpret_cast<float*>(s_rec + BATCH * 3);                       // [BATCH * 9]
-  float* s_x = s_g + BATCH * 9;                                                   // per warp: wG[8][36] | w[8][36]
+  float4* s_rec = smem_f4;                                                        // [BATCH * F4]
+  float* s_g = reinterpret_cast<float*>(s_rec + BATCH * F4);                      // [BATCH * NG]
+  float* s_x = s_g + BATCH * NG;                                                  // per warp: wG[8][36] | w[8][36]
   float* s_cw = s_x + (BLEND_THREADS / 32) * 2 * HITS * XROW;                     // per warp: cotangent weights, hi/lo, A-fragment order
-  float* s_mw = s_cw + (BLEND_THREADS / 32) * 192;                                // per warp: moment weights, A-fragment order
+  float* s_mw = s_cw + (BLEND_THREADS / 32) * NCW;                                // per warp: moment weights, A-fragment order
   unsigned char* s_bits = reinterpret_cast<unsigned char*>(s_mw + (BLEND_THREADS / 32) * 192);      // [BATCH]
   const int tile = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const SubTile st = make_subtile(v, tile, lane, warp);
@@ -368,11 +412,16 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   const int g = lane >> 2, t = lane & 3;        // mma fragment coordinates of this lane
 
   float Rd = 0.f, dp0 = 0.f, dp1 = 0.f, dp2 = 0.f;
+  float dp3 = 0.f, dp4 = 0.f, dp5 = 0.f;         // SIX only
   int last = 0;                                  // REC: list index + 1 of this pixel's last contributor (0: none)
   if (st.inside) {
     const int64_t pix = (int64_t)st.y * v.W + st.x, HW = (int64_t)v.H * v.W;
     dp0 = dL_dimage[pix]; dp1 = dL_dimage[HW + pix]; dp2 = dL_dimage[2 * HW + pix];
     Rd = image[pix] * dp0 + image[HW + pix] * dp1 + image[2 * HW + pix] * dp2;
+    if (SIX) {
+      dp3 = dL_dimage[3 * HW + pix]; dp4 = dL_dimage[4 * HW + pix]; dp5 = dL_dimage[5 * HW + pix];
+      Rd += image[3 * HW + pix] * dp3 + image[4 * HW + pix] * dp4 + image[5 * HW + pix] * dp5;
+    }
     if (REC) last = v.last_contrib[pix];
   }
   // B fragments of the moment weights, per warp in shared memory, lane-major per k-step s (the reading lane l = g*4 + t < 24
@@ -386,17 +435,17 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
     const float f = g_ == 0 ? 1.f : g_ == 1 ? u : g_ == 2 ? vv : g_ == 3 ? u * u : g_ == 4 ? u * vv : vv * vv;
     s_mw[warp * 192 + k] = f;
   }
-  // B fragments of the cotangent weights (columns 0..2 = channel), lane-major per k-step s as above (LDS.128, lanes < 12):
-  // s_cw[(s*12 + c*4 + t)*4 + {0,1,2,3}] = hi(k=t), hi(k=t+4), lo(k=t), lo(k=t+4)
-  const uint32_t cw_addr = pin_reg(smem_u32(s_cw) + (uint32_t)warp * (192 * 4) + (uint32_t)((min(g, 2) * 4 + t) * 16));
+  // B fragments of the cotangent weights (columns 0..NCH-1 = channel), lane-major per k-step s as above (LDS.128, lanes
+  // < 4 NCH): s_cw[(s*4NCH + c*4 + t)*4 + {0,1,2,3}] = hi(k=t), hi(k=t+4), lo(k=t), lo(k=t+4)
+  const uint32_t cw_addr = pin_reg(smem_u32(s_cw) + (uint32_t)warp * (NCW * 4) + (uint32_t)((min(g, NCH - 1) * 4 + t) * 16));
   {
-    float* cw = s_cw + warp * 192;
+    float* cw = s_cw + warp * NCW;
     const int col = lane & 7, s = lane >> 3, tt = col & 3, which = col >> 2;
-    const float dpc[3] = {dp0, dp1, dp2};
+    const float dpc[6] = {dp0, dp1, dp2, dp3, dp4, dp5};
 #pragma unroll
-    for (int c = 0; c < 3; c++) {
-      cw[(s * 12 + c * 4 + tt) * 4 + which] = dpc[c];                   // read as trunc(x) by the tensor core
-      cw[(s * 12 + c * 4 + tt) * 4 + 2 + which] = tf32_lo(dpc[c]);
+    for (int c = 0; c < NCH; c++) {
+      cw[(s * 4 * NCH + c * 4 + tt) * 4 + which] = dpc[c];              // read as trunc(x) by the tensor core
+      cw[(s * 4 * NCH + c * 4 + tt) * 4 + 2 + which] = tf32_lo(dpc[c]);
     }
   }
   __syncwarp();
@@ -416,14 +465,16 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   auto stage = [&]() {
     if (tid < cnt) {
       // REC: walk exactly the (sub-tile, splat) pairs that composited something in the forward
-      stage_splat(s_rec, s_bits, tid, splat, id_next, tx0, ty0, REC ? v.contrib_entry + beg + base + tid : nullptr);
+      stage_splat<SIX>(s_rec, s_bits, tid, splat, id_next, tx0, ty0, REC ? v.contrib_entry + beg + base + tid : nullptr,
+                       v.splat_ext);
 #pragma unroll
-      for (int k = 0; k < 9; k++) s_g[tid * 9 + k] = 0.f;
+      for (int k = 0; k < NG; k++) s_g[tid * NG + k] = 0.f;
     } else {
       s_bits[tid] = 0;
     }
     id_next = base + BATCH + tid < n ? ids[beg + base + BATCH + tid] : -1;
     if (id_next >= 0) prefetch_l2(splat + (int64_t)id_next * LGR_SPLAT_FLOATS);
+    if (SIX && id_next >= 0) prefetch_l2(v.splat_ext + 4 * (int64_t)id_next);
   };
   if (n > 0) stage();
   while (base < n) {
@@ -450,7 +501,7 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
           const int jB = two ? __ffs(mask) - 1 : jA;
           mask &= mask - 1;
           const int eA = c0 + jA, eB = c0 + jB;
-          const uint32_t recA = s_rec_addr + 48u * (uint32_t)eA, recB = s_rec_addr + 48u * (uint32_t)eB;
+          const uint32_t recA = s_rec_addr + RB * (uint32_t)eA, recB = s_rec_addr + RB * (uint32_t)eB;
           const float4 r0A = lds_f4(recA), r0B = lds_f4(recB);
           const float2 r1A = lds_f2(recA + 16u), r1B = lds_f2(recB + 16u);                  // (conic_z, opacity)
           const float dxA = __fsub_rn(r0A.x, pxf), dyA = __fsub_rn(r0A.y, pyf);
@@ -466,7 +517,7 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
             // every visited splat in front of the pixel's last contributor with alpha >= 1/255 was composited by the forward
             // (it would otherwise have stopped the pixel there); same multiplications, so T follows the forward bit for bit
             // (the staged record holds the entry's index in the tile list where the box test's hx was)
-            const int iA = __float_as_int(s_rec[3 * eA + 1].z), iB = __float_as_int(s_rec[3 * eB + 1].z);
+            const int iA = __float_as_int(s_rec[F4 * eA + 1].z), iB = __float_as_int(s_rec[F4 * eB + 1].z);
             cA = !done && powerA <= 0.0f && alphaA >= ALPHA_MIN;
             if (cA) T = __fmul_rn(T, omA);
             done = (iA + 1 >= last);
@@ -491,7 +542,11 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
             if (cA) {
               const float4 r2 = lds_f4(recA + 32u);
               w = alphaA * TA;
-              const float cdot = r2.x * dp0 + r2.y * dp1 + r2.z * dp2;
+              float cdot = r2.x * dp0 + r2.y * dp1 + r2.z * dp2;
+              if (SIX) {
+                const float4 r3 = lds_f4(recA + 48u);
+                cdot += r3.x * dp3 + r3.y * dp4 + r3.z * dp5;
+              }
               Rd = fmaf(-cdot, w, Rd);                          // what is behind the splat (+ bg T_final), dotted with dL/dC
               const float dL_dalpha = cdot * TA - Rd * rcp_approx(omA);
               wG = r1A.y * dL_dalpha * GA;                      // dL/dG * G   (the 0.99 clamp is straight-through)
@@ -506,7 +561,11 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
             if (cB) {
               const float4 r2 = lds_f4(recB + 32u);
               w = alphaB * TB;
-              const float cdot = r2.x * dp0 + r2.y * dp1 + r2.z * dp2;
+              float cdot = r2.x * dp0 + r2.y * dp1 + r2.z * dp2;
+              if (SIX) {
+                const float4 r3 = lds_f4(recB + 48u);
+                cdot += r3.x * dp3 + r3.y * dp4 + r3.z * dp5;
+              }
               Rd = fmaf(-cdot, w, Rd);
               const float dL_dalpha = cdot * TB - Rd * rcp_approx(omB);
               wG = r1B.y * dL_dalpha * GB;
@@ -533,19 +592,24 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
             float2 bm = make_float2(0.f, 0.f);
             float4 bc = make_float4(0.f, 0.f, 0.f, 0.f);
             if (g < 6) bm = lds_f2(mw_addr + 192u * s);
-            if (g < 3) bc = lds_f4(cw_addr + 192u * s);
+            if (g < NCH) bc = lds_f4(cw_addr + (64u * NCH) * s);
             mma_tf32(d0, d1, z0, z1, a0, a1, a2, a3, __float_as_uint(bm.x), __float_as_uint(bm.y));
             mma_tf32(y0, y1, d2, d3, a0, a1, a2, a3, __float_as_uint(bc.x), __float_as_uint(bc.y));
             mma_tf32(d0, d1, z0, z1, l0, l1, l2, l3, __float_as_uint(bm.x), __float_as_uint(bm.y));
             mma_tf32(y0, y1, d2, d3, l0, l1, l2, l3, __float_as_uint(bc.x), __float_as_uint(bc.y));
             mma_tf32(y0, y1, d2, d3, a0, a1, a2, a3, __float_as_uint(bc.z), __float_as_uint(bc.w));
           }
-          // lane (g, t): d0/d1 = moments 2t, 2t+1 of hit g (t < 3) ; d2/d3 = colour sums 2t, 2t+1 of hit g (t = 0: 0, 1; t = 1: 2)
-          const uint32_t acc = s_g_addr + 36u * (uint32_t)__shfl_sync(FULL, my_e, g);
+          // lane (g, t): d0/d1 = moments 2t, 2t+1 of hit g (t < 3) ; d2/d3 = colour sums 2t, 2t+1 of hit g (three channels:
+          // t = 0: 0, 1; t = 1: 2.  SIX: t < 3)
+          const uint32_t acc = s_g_addr + (4u * NG) * (uint32_t)__shfl_sync(FULL, my_e, g);
           if (g < pend) {
             if (t < 3) { red_shared_add_f32(acc + 8u * t, d0); red_shared_add_f32(acc + 8u * t + 4u, d1); }
-            if (t < 2) red_shared_add_f32(acc + 24u + 8u * t, d2);
-            if (t == 0) red_shared_add_f32(acc + 28u, d3);
+            if (SIX) {
+              if (t < 3) { red_shared_add_f32(acc + 24u + 8u * t, d2); red_shared_add_f32(acc + 28u + 8u * t, d3); }
+            } else {
+              if (t < 2) red_shared_add_f32(acc + 24u + 8u * t, d2);
+              if (t == 0) red_shared_add_f32(acc + 28u, d3);
+            }
           }
           __syncwarp();
           pend = 0;
@@ -555,14 +619,15 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
     }
     const int all_done = __syncthreads_and(done);      // B: every warp has left the walk
     if (tid < cnt) {
-      const float* m = s_g + tid * 9;
+      const float* m = s_g + tid * NG;
       const float M00 = m[0], M10 = m[1], M01 = m[2], M20 = m[3], M11 = m[4], M02 = m[5];
-      const bool nz = (M00 != 0.f) | (M10 != 0.f) | (M01 != 0.f) | (M20 != 0.f) | (M11 != 0.f) | (M02 != 0.f) |
-                      (m[6] != 0.f) | (m[7] != 0.f) | (m[8] != 0.f);
+      bool nz = (M00 != 0.f) | (M10 != 0.f) | (M01 != 0.f) | (M20 != 0.f) | (M11 != 0.f) | (M02 != 0.f) |
+                (m[6] != 0.f) | (m[7] != 0.f) | (m[8] != 0.f);
+      if (SIX) nz |= (m[NG - 3] != 0.f) | (m[NG - 2] != 0.f) | (m[NG - 1] != 0.f);
       if (nz) {
-        const float4 r0 = s_rec[3 * tid];
-        const float2 r1 = *reinterpret_cast<const float2*>(&s_rec[3 * tid + 1]);
-        const int id = __float_as_int(s_rec[3 * tid + 2].w);
+        const float4 r0 = s_rec[F4 * tid];
+        const float2 r1 = *reinterpret_cast<const float2*>(&s_rec[F4 * tid + 1]);
+        const int id = __float_as_int(s_rec[F4 * tid + 2].w);
         const float X = r0.x - tcx, Y = r0.y - tcy;
         const float Sx = fmaf(X, M00, -M10), Sy = fmaf(Y, M00, -M01);                       // sum wG dx, sum wG dy
         const float Sxx = fmaf(X, fmaf(X, M00, -2.f * M10), M20);                           // sum wG dx^2
@@ -579,7 +644,8 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
         float4* dst = reinterpret_cast<float4*>(dsplat + (int64_t)id * LGR_GRAD_FLOATS);
         atomicAdd(dst, a);
         atomicAdd(dst + 1, b);
-        atomicAdd(reinterpret_cast<float*>(dst + 2), m[8]);
+        if (SIX) atomicAdd(dst + 2, make_float4(m[8], m[NG - 3], m[NG - 2], m[NG - 1]));      // d/db, d/dc3..5
+        else atomicAdd(reinterpret_cast<float*>(dst + 2), m[8]);
       }
     }
     base += BATCH;
@@ -590,6 +656,20 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
 }
 
 // ---------------------------------------------------------------------------------------------------------
+template <bool SIX>
+static void launch_blend_fwd_ch(const View& v, bool rec, int ntiles, const int32_t* tile_start, const int32_t* sorted_ids,
+                                const float* splat, float* image, float* final_T, int32_t* n_contrib, int32_t* pid_pixel,
+                                float* pw_pixel, unsigned* pwb, int32_t* point_count, cudaStream_t st) {
+  if (v.want_aux && rec)
+    blend_fwd_kernel<true, true, SIX><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
+  else if (v.want_aux)
+    blend_fwd_kernel<true, false, SIX><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
+  else if (rec)
+    blend_fwd_kernel<false, true, SIX><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
+  else
+    blend_fwd_kernel<false, false, SIX><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
+}
+
 int launch_blend_fwd(const View& v, const int32_t* tile_start, const int32_t* sorted_ids, const float* splat,
                      float* image, float* final_T, int32_t* n_contrib, int32_t* pid_pixel, float* pw_pixel,
                      float* point_weight, int32_t* point_count, cudaStream_t st) {
@@ -598,30 +678,36 @@ int launch_blend_fwd(const View& v, const int32_t* tile_start, const int32_t* so
   ProfScope ps(K_BLEND_FWD, st);
   unsigned* pwb = reinterpret_cast<unsigned*>(point_weight);
   const bool rec = v.contrib_id != nullptr && v.contrib_entry != nullptr && v.contrib_count != nullptr;
-  if (v.want_aux && rec)
-    blend_fwd_kernel<true, true><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
-  else if (v.want_aux)
-    blend_fwd_kernel<true, false><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
-  else if (rec)
-    blend_fwd_kernel<false, true><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
+  if (v.num_channels == 6)
+    launch_blend_fwd_ch<true>(v, rec, ntiles, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count, st);
   else
-    blend_fwd_kernel<false, false><<<ntiles, BLEND_THREADS, 0, st>>>(v, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count);
+    launch_blend_fwd_ch<false>(v, rec, ntiles, tile_start, sorted_ids, splat, image, final_T, n_contrib, pid_pixel, pw_pixel, pwb, point_count, st);
   LGR_CHECK_LAUNCH();
   return 0;
+}
+
+template <bool SIX>
+static cudaError_t launch_blend_bwd_ch(const View& v, bool rec, int ntiles, const int32_t* tile_start, const int32_t* sorted_ids,
+                                       const float* splat, const float* image, const float* dL_dimage, float* dsplat, cudaStream_t st) {
+  // > 48 KB of dynamic shared memory needs the opt-in; the attribute is per device and cheap to set, so set it every time
+  constexpr int smem = SIX ? BWD6_SMEM : BWD_SMEM;
+  cudaError_t e = rec ? cudaFuncSetAttribute(blend_bwd_kernel<true, SIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)
+                      : cudaFuncSetAttribute(blend_bwd_kernel<false, SIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return e;
+  ProfScope ps(K_BLEND_BWD, st);
+  if (rec) blend_bwd_kernel<true, SIX><<<ntiles, BLEND_THREADS, smem, st>>>(v, tile_start, sorted_ids, splat, image, dL_dimage, dsplat);
+  else blend_bwd_kernel<false, SIX><<<ntiles, BLEND_THREADS, smem, st>>>(v, tile_start, sorted_ids, splat, image, dL_dimage, dsplat);
+  return cudaSuccess;
 }
 
 int launch_blend_bwd(const View& v, const int32_t* tile_start, const int32_t* sorted_ids, const float* splat,
                      const float* image, const float* dL_dimage, float* dsplat, cudaStream_t st) {
   const int ntiles = v.gx * (v.row1 - v.row0);
   if (ntiles <= 0) return 0;
-  // > 48 KB of dynamic shared memory needs the opt-in; the attribute is per device and cheap to set, so set it every time
   const bool rec = v.contrib_id != nullptr && v.contrib_entry != nullptr && v.contrib_count != nullptr && v.last_contrib != nullptr;
-  cudaError_t e = rec ? cudaFuncSetAttribute(blend_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM)
-                      : cudaFuncSetAttribute(blend_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+  const cudaError_t e = v.num_channels == 6 ? launch_blend_bwd_ch<true>(v, rec, ntiles, tile_start, sorted_ids, splat, image, dL_dimage, dsplat, st)
+                                            : launch_blend_bwd_ch<false>(v, rec, ntiles, tile_start, sorted_ids, splat, image, dL_dimage, dsplat, st);
   if (e != cudaSuccess) return (int)e;
-  ProfScope ps(K_BLEND_BWD, st);
-  if (rec) blend_bwd_kernel<true><<<ntiles, BLEND_THREADS, BWD_SMEM, st>>>(v, tile_start, sorted_ids, splat, image, dL_dimage, dsplat);
-  else blend_bwd_kernel<false><<<ntiles, BLEND_THREADS, BWD_SMEM, st>>>(v, tile_start, sorted_ids, splat, image, dL_dimage, dsplat);
   LGR_CHECK_LAUNCH();
   return 0;
 }

@@ -53,7 +53,16 @@ static bool view_ok(const lgr_view* v) {
     return false;
   const int lists = (v->contrib_id_d != nullptr) + (v->contrib_entry_d != nullptr) + (v->contrib_count_d != nullptr);
   if (lists != 0 && lists != 3) return false;      // the compacted contribution list comes whole or not at all
+  if (v->num_channels != 0 && v->num_channels != 3 && v->num_channels != 6) return false;
+  if (v->num_channels == 6 && !v->splat_ext_d) return false;
   return true;
+}
+
+// Six colour channels (lgr_view.num_channels = 6) exist for precomputed colours on one GPU only: 0 when the view is fine.
+static int six_channels_check(const lgr_view* v) {
+  if (v->num_channels != 6) return 0;
+  if (v->raw_params || v->gather_index_d || v->num_owners > 0 || v->region_count_d || v->pid_map_d) return LGR_E_UNSUPPORTED;
+  return 0;
 }
 
 extern "C" {
@@ -81,6 +90,9 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
                         const float* shs_d, float* splat_d, int32_t* radii_d, uint8_t* clamped_d,
                         int32_t* tile_start_d, int32_t* tile_cursor_d, int32_t* meta_d, void* stream) {
   if (!view_ok(view) || n < 0 || !tile_start_d || !tile_cursor_d || !meta_d) return LGR_E_BADARG;
+  if (const int rc6 = six_channels_check(view)) return rc6;
+  if (view->num_channels == 6 && shs_d) return LGR_E_UNSUPPORTED;
+  if (view->num_channels == 6 && n > 0 && !colors_precomp_d) return LGR_E_BADARG;
   // colour sources: colors_precomp XOR shs (stock), or -- with raw_params -- raw DC colours + the rest coefficients
   // (LoG's colour activation fused, activation.py:27-34)
   const bool log_sh = view->raw_params && colors_precomp_d && shs_d;
@@ -129,6 +141,7 @@ int lgr_forward_render(const lgr_view* view, int64_t n, int64_t num_instances, i
       !n_contrib_d)
     return LGR_E_BADARG;
   if (num_instances > 0 && (!inst_key_d || !inst_val_d || !sorted_ids_d || !splat_d || !radii_d)) return LGR_E_BADARG;
+  if (const int rc6 = six_channels_check(view)) return rc6;
   if (view->want_aux && (!point_id_pixel_d || !point_weight_pixel_d || (n > 0 && !point_weight_d))) return LGR_E_BADARG;
   if (num_instances > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
   if (view->contrib_id_d && max_tile_len > LGR_CONTRIB_MAX_LIST) return LGR_E_UNSUPPORTED;      // list indices would not fit
@@ -151,6 +164,7 @@ int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t ins
       !n_contrib_d || !inst_key_d || !inst_val_d || !sorted_ids_d)
     return LGR_E_BADARG;
   if (n > 0 && (!splat_d || !radii_d)) return LGR_E_BADARG;
+  if (const int rc6 = six_channels_check(view)) return rc6;
   if (view->want_aux && (!point_id_pixel_d || !point_weight_pixel_d || (n > 0 && !point_weight_d))) return LGR_E_BADARG;
   if (instance_capacity > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
   // contrib_entry_d's list indices: a list longer than lgr_sort_smem_capacity() (far below LGR_CONTRIB_MAX_LIST) already
@@ -173,6 +187,8 @@ int lgr_backward(const lgr_view* view, int64_t n, int64_t num_instances, const f
                  float* dcolors_d, float* dshs_d, float* grad_rows_d, void* const* peer_stage_d, int32_t my_rank,
                  int64_t num_rows, void* stream) {
   if (!view_ok(view) || n < 0 || !tile_start_d || !image_d || !dL_dimage_d) return LGR_E_BADARG;
+  if (const int rc6 = six_channels_check(view)) return rc6;
+  if (view->num_channels == 6 && (shs_d || grad_rows_d || peer_stage_d)) return LGR_E_UNSUPPORTED;
   if (n == 0) return 0;
   const bool log_sh = view->raw_params && colors_precomp_d && shs_d;      // LoG-style SH: DC colours + rest coefficients
   const bool use_sh = shs_d != nullptr && !log_sh;
@@ -253,6 +269,7 @@ int lgr_shard_send(const lgr_view* view, const lgr_shard_layout* layout, int64_t
                    const float* splat_d, const int32_t* radii_d, int32_t* send_scratch_d, void* const* peer_base_d,
                    void* stream) {
   if (!view_ok(view) || !layout_ok(layout) || n_local < 0 || gid_base < 0 || !send_scratch_d || !peer_base_d) return LGR_E_BADARG;
+  if (view->num_channels == 6) return LGR_E_UNSUPPORTED;      // shard mode moves 12-float records only
   if (n_local > layout->cap || (n_local > 0 && (!splat_d || !radii_d))) return LGR_E_BADARG;
   if (view->num_owners != 0 || view->tile_row_begin != 0 || (view->tile_row_end != 0 && view->tile_row_end != (view->image_height + TILE - 1) / TILE))
     return LGR_E_BADARG;      // the source side works on the full image
@@ -270,6 +287,7 @@ int lgr_shard_recv_bin_aux(const lgr_view* view, const lgr_shard_layout* layout,
                            int32_t* tile_start_d, int32_t* tile_cursor_d, int32_t* meta_d, float* point_weight_rows_d,
                            int32_t* point_count_rows_d, void* stream) {
   if (!view_ok(view) || !layout_ok(layout) || !exchange_d || !dsplat_d || !tile_start_d || !tile_cursor_d || !meta_d) return LGR_E_BADARG;
+  if (view->num_channels == 6) return LGR_E_UNSUPPORTED;      // shard mode moves 12-float records only
   if (view->num_owners != 0) return LGR_E_BADARG;
   // the view must carry the layout's region map: this call and the render that follows visit the used rows only
   if (view->region_count_d != reinterpret_cast<const int32_t*>(exchange_d + layout->off_count) || view->region_cap != layout->cap ||
@@ -293,6 +311,7 @@ int lgr_blend_backward(const lgr_view* view, int64_t n, int64_t num_instances, c
                        const int32_t* tile_start_d, const int32_t* sorted_ids_d, const float* image_d,
                        const float* dL_dimage_d, float* dsplat_d, void* stream) {
   if (!view_ok(view) || n < 0 || num_instances < 0 || !tile_start_d || !image_d || !dL_dimage_d) return LGR_E_BADARG;
+  if (const int rc6 = six_channels_check(view)) return rc6;
   if (num_instances == 0 || n == 0) return 0;
   if (!splat_d || !sorted_ids_d || !dsplat_d) return LGR_E_BADARG;
   return launch_blend_bwd(make_view(view, n), tile_start_d, sorted_ids_d, splat_d, image_d, dL_dimage_d, dsplat_d,
@@ -311,6 +330,7 @@ int lgr_shard_gather(const lgr_view* view, const lgr_shard_layout* layout, int64
                      const int32_t* radii_d, const int32_t* send_scratch_d, const float* exchange_d,
                      float* dsplat_local_d, float* point_weight_d, int32_t* point_count_d, void* stream) {
   if (!view_ok(view) || !layout_ok(layout) || n_local < 0 || n_local > layout->cap) return LGR_E_BADARG;
+  if (view->num_channels == 6) return LGR_E_UNSUPPORTED;      // shard mode moves 12-float records only
   if (n_local == 0) return 0;
   if (!splat_d || !radii_d || !send_scratch_d || !exchange_d || !dsplat_local_d) return LGR_E_BADARG;
   return launch_shard_gather(make_view(view, n_local), make_layout(layout), n_local, splat_d, radii_d, send_scratch_d, exchange_d,
@@ -321,6 +341,7 @@ int lgr_shard_gather_packed(const lgr_view* view, const lgr_shard_layout* layout
                             const int32_t* radii_d, const int32_t* send_scratch_d, const float* exchange_d,
                             float* dsplat_local_d, float* point_weight_d, int32_t* point_count_d, void* stream) {
   if (!view_ok(view) || !layout_ok(layout) || n_local < 0 || n_local > layout->cap) return LGR_E_BADARG;
+  if (view->num_channels == 6) return LGR_E_UNSUPPORTED;      // shard mode moves 12-float records only
   if (n_local == 0) return 0;
   if (!splat_d || !radii_d || !send_scratch_d || !exchange_d || !dsplat_local_d) return LGR_E_BADARG;
   return launch_shard_gather(make_view(view, n_local), make_layout(layout), n_local, splat_d, radii_d, send_scratch_d, exchange_d,

@@ -51,6 +51,8 @@ struct View {
   const float* proj;
   const float* campos;
   const float* bg;
+  int num_channels;          // 3, or 6: colors_precomp (N,6), image (6,H,W); channels 3..5 travel in splat_ext
+  float* splat_ext;          // (N,4) with 6 channels: the projected record's fourth float4, (c3, c4, c5, 0)
 };
 
 inline View make_view(const lgr_view* v, int64_t n = 0) {
@@ -71,6 +73,7 @@ inline View make_view(const lgr_view* v, int64_t n = 0) {
   o.sh_degree = v->sh_degree; o.sh_K = v->sh_coeffs; o.filter_mode = v->filter_mode; o.want_aux = v->want_aux;
   o.raw_params = v->raw_params;
   o.view = v->viewmatrix_d; o.proj = v->projmatrix_d; o.campos = v->campos_d; o.bg = v->bg_d;
+  o.num_channels = v->num_channels == 6 ? 6 : 3; o.splat_ext = v->splat_ext_d;
   return o;
 }
 

@@ -59,7 +59,8 @@ compute_radius_kernel(int64_t n, const float* __restrict__ means, const float* _
 // rgb = SH2RGB(dc) + eval_sh_wobase(dir, rest, degree) with dc = `colors` (N,3) raw and rest = `shs` (N,K,3); unlike the
 // stock SH path there is NO clamp at 0 and the direction comes from the DETACHED position (no gradient to the mean).
 // COV3D: the world-space covariance comes precomputed from View::cov3d (stock cov3D_precomp) instead of scales / rotations.
-template <bool USE_SH, bool LOG_SH = false, bool COV3D = false>
+// SIX: six precomputed colour channels, `colors` (N,6); channels 3..5 go to View::splat_ext (N,4) as (c3, c4, c5, 0).
+template <bool USE_SH, bool LOG_SH = false, bool COV3D = false, bool SIX = false>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
                    const float* __restrict__ scales, const float* __restrict__ rots,
@@ -165,7 +166,7 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     cov2d(sV, p, Sg, v.fx, v.fy, v.tanfovx, v.tanfovy, v.filter_mode, cv);
     float det;
     const float radf = radius_from_cov(cv.a, cv.b, cv.c, det);
-    float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0, r2 = r0;
+    float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0, r2 = r0, r3 = r0;
     if (cv.t[2] > NEAR_Z && det > 0.0f) {
       float hom[4];
 #pragma unroll
@@ -206,6 +207,10 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
 #pragma unroll
           for (int ch = 0; ch < 3; ch++) if (rgb[ch] < 0.0f) { cl |= (uint8_t)(1u << ch); rgb[ch] = 0.0f; }
           clamped[i] = cl;
+        } else if (SIX) {      // no raw_params, no gather (checked by the caller)
+          const float* c6 = colors + 6 * src;
+          rgb[0] = __ldg(c6); rgb[1] = __ldg(c6 + 1); rgb[2] = __ldg(c6 + 2);
+          r3 = make_float4(__ldg(c6 + 3), __ldg(c6 + 4), __ldg(c6 + 5), 0.f);
         } else {
           load3(colors, src, rgb);
           if (v.raw_params) {      // SH2RGB (sh_utils.py:72-73)
@@ -240,6 +245,7 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     if (v.num_owners == 0 || in_band) {      // band mode: records outside the band are never read
       float4* dst = reinterpret_cast<float4*>(splat + i * LGR_SPLAT_FLOATS);
       dst[0] = r0; dst[1] = r1; dst[2] = r2;
+      if (SIX) reinterpret_cast<float4*>(v.splat_ext)[i] = r3;
     }
     radii[i] = rad_out;
     if (USE_SH && rad_out == 0) clamped[i] = 0;
@@ -279,7 +285,8 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
 // ---------------------------------------------------------------------------------------------------------
 // backward projection: dsplat (d/dpx, d/dpy, d/dconic xyz, d/dopacity, d/drgb) -> input gradients
 // ---------------------------------------------------------------------------------------------------------
-template <bool USE_SH, bool ROWS, bool LOG_SH = false, bool COV3D = false>
+// SIX: six precomputed colour channels; d/dc3..5 are floats 9..11 of the dsplat row, dcolors is (N,6).
+template <bool USE_SH, bool ROWS, bool LOG_SH = false, bool COV3D = false, bool SIX = false>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
                    const float* __restrict__ scales, const float* __restrict__ rots, const float* __restrict__ shs, const int32_t* __restrict__ radii,
@@ -309,7 +316,7 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     i = v.band_rows[row];
   }
   float dm[3] = {0.f, 0.f, 0.f}, dm2[2] = {0.f, 0.f}, dop = 0.f, dsc[3] = {0.f, 0.f, 0.f}, dq[4] = {0.f, 0.f, 0.f, 0.f};
-  float drgb[3] = {0.f, 0.f, 0.f};
+  float drgb[3] = {0.f, 0.f, 0.f}, dext[3] = {0.f, 0.f, 0.f};
   const bool live = active && radii[i] > 0;
   const int64_t src = (v.gather && live) ? v.gather[i] : i;      // gather-fused call: inputs come from row gather[i] of the tables
   const int K = v.sh_K;
@@ -342,6 +349,7 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     cov2d(sV, p, Sg, v.fx, v.fy, v.tanfovx, v.tanfovy, v.filter_mode, cv);
     dop = g1.y;
     drgb[0] = g1.z; drgb[1] = g1.w; drgb[2] = g2.x;
+    if (SIX) { dext[0] = g2.y; dext[1] = g2.z; dext[2] = g2.w; }
     // conic -> cov2D (true derivatives; d/dconic_y is w.r.t. the single off-diagonal parameter)
     const float a = cv.a, b = cv.b, c = cv.c;
     const float det = a * c - b * b, idet2 = 1.0f / (det * det);
@@ -547,7 +555,12 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     dscales[3 * i] = dsc[0]; dscales[3 * i + 1] = dsc[1]; dscales[3 * i + 2] = dsc[2];
     reinterpret_cast<float4*>(drots)[i] = make_float4(dq[0], dq[1], dq[2], dq[3]);
   }
-  if (!USE_SH) { dcolors[3 * i] = drgb[0]; dcolors[3 * i + 1] = drgb[1]; dcolors[3 * i + 2] = drgb[2]; }
+  if (SIX) {
+    float* dc = dcolors + 6 * i;
+    dc[0] = drgb[0]; dc[1] = drgb[1]; dc[2] = drgb[2]; dc[3] = dext[0]; dc[4] = dext[1]; dc[5] = dext[2];
+  } else if (!USE_SH) {
+    dcolors[3 * i] = drgb[0]; dcolors[3 * i + 1] = drgb[1]; dcolors[3 * i + 2] = drgb[2];
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -691,7 +704,11 @@ int launch_project_fwd(const View& v, int64_t n, const float* means, const float
   if (n == 0) return 0;
   const unsigned blocks = (unsigned)((n + PROJ_THREADS - 1) / PROJ_THREADS);
   ProfScope ps(K_PROJECT_FWD, st);
-  if (v.cov3d && colors)      // stock cov3D_precomp (checked by the caller: no raw_params, no band mode)
+  if (v.num_channels == 6 && v.cov3d)      // six colour channels (checked by the caller: colors only, no raw_params / gather / band)
+    project_fwd_kernel<false, false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+  else if (v.num_channels == 6)
+    project_fwd_kernel<false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+  else if (v.cov3d && colors)      // stock cov3D_precomp (checked by the caller: no raw_params, no band mode)
     project_fwd_kernel<false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
   else if (v.cov3d)
     project_fwd_kernel<true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
@@ -716,7 +733,11 @@ int launch_project_bwd(const View& v, int64_t n, const float* means, const float
   if (n == 0) return 0;
   const unsigned blocks = (unsigned)((n + PROJ_THREADS - 1) / PROJ_THREADS);
   ProfScope ps(K_PROJECT_BWD, st);
-  if (v.cov3d && !use_sh)
+  if (v.num_channels == 6 && v.cov3d)
+    project_bwd_kernel<false, false, false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+  else if (v.num_channels == 6)
+    project_bwd_kernel<false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+  else if (v.cov3d && !use_sh)
     project_bwd_kernel<false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
   else if (v.cov3d)
     project_bwd_kernel<true, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);

@@ -77,7 +77,7 @@ def _stream(device=None):
 
 def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: bool, sh_coeffs: int, tile_rows, keep,
                num_owners=0, band_ids=None, band_count=None, band_blk=None, band_rows=None, band_dsplat=None,
-               raw_params=False, tile_rank=None, gather_index=None, pid_map=None, cov3D_precomp=None):
+               raw_params=False, tile_rank=None, gather_index=None, pid_map=None, cov3D_precomp=None, splat_ext=None):
     dev = s.viewmatrix.device
     vm, pm = _f32c(s.viewmatrix, 'viewmatrix'), _f32c(s.projmatrix, 'projmatrix', dev)
     bg = _f32c(s.bg, 'bg', dev)
@@ -101,6 +101,8 @@ def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: boo
     v.gather_index_d = gather_index.data_ptr() if gather_index is not None else None
     v.pid_map_d = pid_map.data_ptr() if pid_map is not None else None
     v.cov3D_precomp_d = cov3D_precomp.data_ptr() if cov3D_precomp is not None else None
+    if splat_ext is not None:      # six colour channels: channels 3..5 of every projected record live in splat_ext (N,4)
+        v.num_channels, v.splat_ext_d = 6, splat_ext.data_ptr()
     v.viewmatrix_d, v.projmatrix_d = vm.data_ptr(), pm.data_ptr()
     v.campos_d = cp.data_ptr() if cp is not None else None
     v.bg_d = bg.data_ptr()
@@ -119,6 +121,28 @@ def set_contrib_lists(view, buf, D, n_contrib):
     view.last_contrib_d = n_contrib.data_ptr()
 
 
+def colour_channels(colors_precomp, settings, shs=None, raw_params=False, gather_index=None, num_owners=0):
+    """Number of precomputed colour channels of a call: 3, or 6 for colors_precomp (N,6), which composites six channels in
+    one pass (e.g. LoG's colour and its (depth, height, 1) pass).  Raises for any other width and for the combinations
+    six channels do not support."""
+    if colors_precomp is None:
+        return 3
+    width = int(colors_precomp.shape[-1]) if colors_precomp.dim() > 0 else 0
+    if width not in (3, 6):
+        raise _capi.LgrError(f'colors_precomp must have 3 or 6 channels per Gaussian, got shape {tuple(colors_precomp.shape)}')
+    if width == 3:
+        return 3
+    if colors_precomp.dim() != 2:
+        raise _capi.LgrError(f'six-channel colors_precomp must be (N,6), got shape {tuple(colors_precomp.shape)}')
+    for what, used in (('shs', shs is not None), ('raw_params', raw_params), ('gather_index (render_gathered)', gather_index is not None),
+                       ('band mode (num_owners > 0)', num_owners > 0)):
+        if used:
+            raise _capi.LgrError(f'six colour channels (colors_precomp (N,6)) are not available with {what}')
+    if settings.bg.numel() != 6:
+        raise _capi.LgrError(f'six colour channels need a background of 6 entries (raster_settings.bg), got {settings.bg.numel()}')
+    return 6
+
+
 def use_contrib_lists(D, max_tile_len):
     """Record the contribution lists for the backward?  (Not for an empty view, nor for a tile list longer than the entry
     word's index field; max_tile_len None: a device-sized call, whose lists are bounded by lgr_sort_smem_capacity().)"""
@@ -129,7 +153,8 @@ class RasterState:
     """Buffers produced by the forward and consumed by the backward (kept alive by autograd)."""
     __slots__ = ('view', 'keep', 'n', 'num_instances', 'max_tile_len', 'stock_instances', 'num_visible', 'splat',
                  'radii', 'clamped', 'tile_start', 'sorted_ids', 'final_T', 'n_contrib', 'image', 'sh', 'num_owners',
-                 'band_ids', 'band_count', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D', 'contrib')
+                 'band_ids', 'band_count', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D', 'contrib',
+                 'channels', 'splat_ext')
 
     def read_stats(self):
         """Counters of this forward, read back from meta_d (synchronises): D, longest tile list, D by the stock rule, visible
@@ -159,7 +184,10 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     With raw_params and BOTH colors_precomp (raw DC, (N,3)) and shs (the rest coefficients, (N,K,3)) LoG's whole colour
     activation is fused: SH2RGB(dc) + eval_sh_wobase(dir, shs, settings.sh_degree), no clamp, direction detached.
     cov3D_precomp (N,6): the stock API's precomputed world-space covariance (xx xy xz yy yz zz) instead of scales / rotations
-    (pass those as None); the backward then returns its gradient in state.dcov3D."""
+    (pass those as None); the backward then returns its gradient in state.dcov3D.
+    colors_precomp (N,6) with a 6-entry settings.bg: six channels composited in one pass, image (6,H,W); channels 0..2 equal a
+    call with colors_precomp[:, :3] and bg[:3] bit for bit, channels 3..5 one with [:, 3:] and bg[3:]."""
+    channels = colour_channels(colors_precomp, settings, shs, raw_params, gather_index, num_owners)
     lib = _capi.load()
     dev = means3D.device
     if cov3D_precomp is not None and (raw_params or num_owners > 0):
@@ -197,8 +225,10 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         band_count = torch.empty((num_owners,), dtype=torch.int32, device=dev)
     tile_rank = torch.empty((max(n, 1), 4), dtype=torch.int32, device=dev) if RANKED_BIN else None
     keep.append(tile_rank)
+    splat_ext = torch.empty((n, 4), dtype=torch.float32, device=dev) if channels == 6 else None
+    keep.append(splat_ext)
     view = _make_view(settings, filter_mode, want_aux, K, tile_rows, keep, num_owners, band_ids, band_count, band_blk, band_rows, band_dsplat,
-                      raw_params, tile_rank, gather_index, cov3D_precomp=cov3D_precomp)
+                      raw_params, tile_rank, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext)
     H, W = view.image_height, view.image_width
     gx, gy = (W + 15) // 16, (H + 15) // 16
     rows = gy if tile_rows is None else int(tile_rows[1]) - int(tile_rows[0])
@@ -218,7 +248,7 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
                 'lgr_forward_project')
     u32 = dict(dtype=torch.int32, device=dev)
     # a sharded call owns only its rows; untouched rows stay zero so that ranks can be summed
-    image = torch.empty((3, H, W), **f32) if tile_rows is None else torch.zeros((3, H, W), **f32)
+    image = torch.empty((channels, H, W), **f32) if tile_rows is None else torch.zeros((channels, H, W), **f32)
     final_T = torch.empty((H, W), **f32) if tile_rows is None else torch.ones((H, W), **f32)
     n_contrib = torch.empty((H, W), **i32) if tile_rows is None else torch.zeros((H, W), **i32)
     pid = pwp = pw = pc = None
@@ -269,6 +299,7 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     s.final_T, s.n_contrib, s.image, s.sh = final_T, n_contrib, image, shs is not None
     s.point_count = pc
     s.contrib = contrib
+    s.channels, s.splat_ext = channels, splat_ext
     s.num_owners, s.band_ids, s.band_count = num_owners, (band_ids, band_blk, band_rows, band_dsplat), band_count
     s.band_counts_host = [int(x) for x in m[_capi.LGR_META_INTS:]] if num_owners > 0 else None
     return image, radii, pid, pwp, pw, s
@@ -314,7 +345,7 @@ def rasterize_backward(state: RasterState, grad_image, means3D, opacities, scale
     if cov:      # stock cov3D_precomp: the covariance gradient replaces the scale / rotation gradients
         state.dcov3D = torch.empty((n, 6), **f32)
         state.view.dcov3D_d = state.dcov3D.data_ptr()
-    dcolors = torch.empty((n, 3), **f32) if colors_precomp is not None else None
+    dcolors = torch.empty((n, state.channels), **f32) if colors_precomp is not None else None
     dshs = torch.empty((n,) + tuple(shs.shape[1:]), **f32) if shs is not None else None
     _capi.check(lib.lgr_backward(ctypes.byref(state.view), n, state.num_instances, _ptr(means3D), _ptr(opacities),
                                  _ptr(scales), _ptr(rotations), _ptr(colors_precomp), _ptr(shs), _ptr(state.splat),

@@ -274,6 +274,8 @@ class SplatExchange:
         from . import _capi
         from .rasterizer import _f32c, _make_view, _ptr, _stream
         lib = _capi.load()
+        if colors_precomp is not None and int(colors_precomp.shape[-1]) != 3:
+            raise _capi.LgrError(f'shard mode renders three precomputed colour channels, got colors_precomp {tuple(colors_precomp.shape)}')
         filter_mode = _capi.LGR_FILTER_MAX if filter_mode is None else filter_mode
         dev = self.buf.device
         n = int(means3D.shape[0])
