@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 18
+#define LGR_ABI_VERSION 19
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -113,7 +113,18 @@ typedef struct lgr_view {
                             (N,6), image_d, dL_dimage_d (6,H,W), bg_d (6,), dcolors_d (N,6), and splat_ext_d is required.
                             Channels 0..2 equal, bit for bit, a 3-channel call with colours [:, :3] and bg[:3]; channels
                             3..5 one with [:, 3:] and bg[3:].  Not available with shs_d, raw_params, gather_index_d, band
-                            mode (num_owners > 0) or shard mode (region_count_d, pid_map_d, lgr_shard_*): LGR_E_UNSUPPORTED. */
+                            mode (num_owners > 0) or shard mode (region_count_d, pid_map_d, lgr_shard_*): LGR_E_UNSUPPORTED
+                            (with log_depth = 0). */
+  int32_t log_depth;     /* 0 or 1.  1: LoG's depth pass (renderer.py:186-201) in the same call, for any colour source
+                            (colors_precomp (N,3), shs, raw_params with or without the rest coefficients, gather_index_d,
+                            cov3D_precomp_d).  The projection generates channels 3..5 per Gaussian as (view depth, world z,
+                            1): the unclamped view-space z of the mean (splat record float 11), means3D z, and 1.  Requires
+                            num_channels = 6 and splat_ext_d (else LGR_E_BADARG); image_d, dL_dimage_d (6,H,W) and bg_d (6,)
+                            as for any six-channel call, but colors_precomp_d and dcolors_d keep their three-channel shapes
+                            (or are NULL with shs).  The backward adds d/d(height) to dmeans3D z and drops d/d(depth) (LoG
+                            computes it from the detached mean) and d/d(1).  Channels 0..2 equal the same call without the
+                            depth pass bit for bit.  Not available in band mode or shard mode (num_owners > 0,
+                            region_count_d, pid_map_d, lgr_shard_*): LGR_E_UNSUPPORTED. */
   float* splat_ext_d;    /* (N,4) or NULL: with num_channels = 6, the fourth float4 of every projected record, (c3, c4, c5, 0),
                             written by lgr_forward_project and read by lgr_forward_render[_device_sized] / lgr_backward /
                             lgr_blend_backward.  The (N,12) splat record (read by the bin and sort kernels) is unchanged. */
@@ -155,7 +166,8 @@ int lgr_mark_visible(int64_t n, const float* means3D_d, const float* viewmatrix_
 
 /* Stage 1 of the forward: per-Gaussian projection + EWA covariance + colour, tile counting, tile scan.
  *   in : means3D (N,3) opacities (N) scales (N,3) rotations (N,4); colors_precomp (N,3) XOR shs (N,K,3)
- *        (colors_precomp (N,6) with view->num_channels = 6; splat_ext_d then receives (N,4))
+ *        (colors_precomp (N,6) with view->num_channels = 6; splat_ext_d then receives (N,4); with view->log_depth = 1
+ *        any colour source, and splat_ext_d receives (view depth, world z, 1, 0))
  *   out: splat_d (N,12) radii_d (N) int32; clamped_d (N) uint8 (SH only, may be NULL with colors_precomp);
  *        tile_start_d (tiles+1) int32 exclusive scan of per-tile counts (tiles = gx * rows rendered);
  *        tile_cursor_d (LGR_TILE_SCRATCH_INTS*tiles) int32 scratch; meta_d (LGR_META_INTS) int32.
@@ -202,7 +214,8 @@ int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t ins
  *   image_d (3,H,W): the forward's output, unmodified.  dsplat_d (N,12) scratch, zero-filled by the caller.
  *   out (each written for every Gaussian; culled ones get 0): dmeans3D (N,3) dmeans2D (N,3; d/d(ndc x,y), z = 0)
  *        dopacities (N) dscales (N,3) drotations (N,4) and dcolors (N,3) XOR dshs (N,K,3).
- *   With view->num_channels = 6: image_d / dL_dimage_d (6,H,W), dcolors_d (N,6); dsplat_d floats 9..11 carry d/dc3..5. */
+ *   With view->num_channels = 6: image_d / dL_dimage_d (6,H,W), dcolors_d (N,6); dsplat_d floats 9..11 carry d/dc3..5.
+ *   With view->log_depth = 1: image_d / dL_dimage_d (6,H,W), dcolors_d (N,3) or dshs_d as without it. */
 int lgr_backward(const lgr_view* view, int64_t n, int64_t num_instances, const float* means3D_d,
                  const float* opacities_d, const float* scales_d, const float* rotations_d,
                  const float* colors_precomp_d, const float* shs_d, const float* splat_d, const int32_t* radii_d,

@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 18
+LGR_ABI_VERSION = 19
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -31,7 +31,7 @@ class LgrView(ctypes.Structure):
                 ('scale_modifier', _f32), ('sh_degree', _i32), ('sh_coeffs', _i32), ('filter_mode', _i32),
                 ('want_aux', _i32), ('tile_row_begin', _i32), ('tile_row_end', _i32),
                 ('num_owners', _i32), ('raw_params', _i32), ('band_ids_d', _vp), ('band_blk_d', _vp), ('band_count_d', _vp), ('band_rows_d', _vp), ('band_dsplat_d', _vp), ('tile_rank_d', _vp), ('gather_index_d', _vp), ('pid_map_d', _vp), ('contrib_id_d', _vp), ('contrib_entry_d', _vp), ('contrib_count_d', _vp), ('last_contrib_d', _vp),
-                ('region_count_d', _vp), ('region_cap', _i64), ('num_regions', _i32), ('num_channels', _i32), ('splat_ext_d', _vp), ('cov3D_precomp_d', _vp), ('dcov3D_d', _vp),
+                ('region_count_d', _vp), ('region_cap', _i64), ('num_regions', _i32), ('num_channels', _i32), ('log_depth', _i32), ('splat_ext_d', _vp), ('cov3D_precomp_d', _vp), ('dcov3D_d', _vp),
                 ('viewmatrix_d', _vp), ('projmatrix_d', _vp), ('campos_d', _vp), ('bg_d', _vp)]
 
 

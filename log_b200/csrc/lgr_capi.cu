@@ -55,13 +55,16 @@ static bool view_ok(const lgr_view* v) {
   if (lists != 0 && lists != 3) return false;      // the compacted contribution list comes whole or not at all
   if (v->num_channels != 0 && v->num_channels != 3 && v->num_channels != 6) return false;
   if (v->num_channels == 6 && !v->splat_ext_d) return false;
+  if (v->log_depth != 0 && (v->log_depth != 1 || v->num_channels != 6)) return false;      // the depth pass is six channels
   return true;
 }
 
-// Six colour channels (lgr_view.num_channels = 6) exist for precomputed colours on one GPU only: 0 when the view is fine.
+// Six colour channels (lgr_view.num_channels = 6) exist on one GPU only, and for precomputed colours only unless the
+// projection generates channels 3..5 (log_depth): 0 when the view is fine.
 static int six_channels_check(const lgr_view* v) {
   if (v->num_channels != 6) return 0;
-  if (v->raw_params || v->gather_index_d || v->num_owners > 0 || v->region_count_d || v->pid_map_d) return LGR_E_UNSUPPORTED;
+  if (v->num_owners > 0 || v->region_count_d || v->pid_map_d) return LGR_E_UNSUPPORTED;
+  if (!v->log_depth && (v->raw_params || v->gather_index_d)) return LGR_E_UNSUPPORTED;
   return 0;
 }
 
@@ -91,8 +94,9 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
                         int32_t* tile_start_d, int32_t* tile_cursor_d, int32_t* meta_d, void* stream) {
   if (!view_ok(view) || n < 0 || !tile_start_d || !tile_cursor_d || !meta_d) return LGR_E_BADARG;
   if (const int rc6 = six_channels_check(view)) return rc6;
-  if (view->num_channels == 6 && shs_d) return LGR_E_UNSUPPORTED;
-  if (view->num_channels == 6 && n > 0 && !colors_precomp_d) return LGR_E_BADARG;
+  const bool six_precomp = view->num_channels == 6 && !view->log_depth;      // colors_precomp (N,6)
+  if (six_precomp && shs_d) return LGR_E_UNSUPPORTED;
+  if (six_precomp && n > 0 && !colors_precomp_d) return LGR_E_BADARG;
   // colour sources: colors_precomp XOR shs (stock), or -- with raw_params -- raw DC colours + the rest coefficients
   // (LoG's colour activation fused, activation.py:27-34)
   const bool log_sh = view->raw_params && colors_precomp_d && shs_d;
@@ -188,7 +192,7 @@ int lgr_backward(const lgr_view* view, int64_t n, int64_t num_instances, const f
                  int64_t num_rows, void* stream) {
   if (!view_ok(view) || n < 0 || !tile_start_d || !image_d || !dL_dimage_d) return LGR_E_BADARG;
   if (const int rc6 = six_channels_check(view)) return rc6;
-  if (view->num_channels == 6 && (shs_d || grad_rows_d || peer_stage_d)) return LGR_E_UNSUPPORTED;
+  if (view->num_channels == 6 && ((shs_d && !view->log_depth) || grad_rows_d || peer_stage_d)) return LGR_E_UNSUPPORTED;
   if (n == 0) return 0;
   const bool log_sh = view->raw_params && colors_precomp_d && shs_d;      // LoG-style SH: DC colours + rest coefficients
   const bool use_sh = shs_d != nullptr && !log_sh;

@@ -60,7 +60,10 @@ compute_radius_kernel(int64_t n, const float* __restrict__ means, const float* _
 // stock SH path there is NO clamp at 0 and the direction comes from the DETACHED position (no gradient to the mean).
 // COV3D: the world-space covariance comes precomputed from View::cov3d (stock cov3D_precomp) instead of scales / rotations.
 // SIX: six precomputed colour channels, `colors` (N,6); channels 3..5 go to View::splat_ext (N,4) as (c3, c4, c5, 0).
-template <bool USE_SH, bool LOG_SH = false, bool COV3D = false, bool SIX = false>
+// DEPTH (View::log_depth): channels 3..5 are LoG's depth-pass colours (renderer.py:186-201), generated here for any colour
+// source: (view depth, world z, 1) -> View::splat_ext as (t_z, p_z, 1, 0); t_z is the unclamped view-space z of the mean
+// (cov2d's t[2], record float 11).
+template <bool USE_SH, bool LOG_SH = false, bool COV3D = false, bool SIX = false, bool DEPTH = false>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
                    const float* __restrict__ scales, const float* __restrict__ rots,
@@ -235,6 +238,7 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
         r0 = make_float4(px, py, cv.c * kdet, -cv.b * kdet);
         r1 = make_float4(cv.a * kdet, o, hx, hy);
         r2 = make_float4(rgb[0], rgb[1], rgb[2], cv.t[2]);
+        if (DEPTH) r3 = make_float4(cv.t[2], p[2], 1.0f, 0.f);
         if (reach) {
           tile_rect_tight(px, py, rad, hx, hy, v.gx, v.gy, v.row0, v.row1, x0, y0, x1, y1);
           big_splat = count_small_tiles(v, tile_count, i, x0, y0, x1, y1);
@@ -245,7 +249,7 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     if (v.num_owners == 0 || in_band) {      // band mode: records outside the band are never read
       float4* dst = reinterpret_cast<float4*>(splat + i * LGR_SPLAT_FLOATS);
       dst[0] = r0; dst[1] = r1; dst[2] = r2;
-      if (SIX) reinterpret_cast<float4*>(v.splat_ext)[i] = r3;
+      if (SIX || DEPTH) reinterpret_cast<float4*>(v.splat_ext)[i] = r3;
     }
     radii[i] = rad_out;
     if (USE_SH && rad_out == 0) clamped[i] = 0;
@@ -286,7 +290,9 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
 // backward projection: dsplat (d/dpx, d/dpy, d/dconic xyz, d/dopacity, d/drgb) -> input gradients
 // ---------------------------------------------------------------------------------------------------------
 // SIX: six precomputed colour channels; d/dc3..5 are floats 9..11 of the dsplat row, dcolors is (N,6).
-template <bool USE_SH, bool ROWS, bool LOG_SH = false, bool COV3D = false, bool SIX = false>
+// DEPTH (View::log_depth): channels 3..5 were generated as (view depth, world z, 1).  d/dc4 (height = the mean's z) goes to
+// dmeans3D z; d/dc3 is dropped (LoG computes the depth from the detached mean) and so is d/dc5 (a constant).
+template <bool USE_SH, bool ROWS, bool LOG_SH = false, bool COV3D = false, bool SIX = false, bool DEPTH = false>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
                    const float* __restrict__ scales, const float* __restrict__ rots, const float* __restrict__ shs, const int32_t* __restrict__ radii,
@@ -427,6 +433,7 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     const float dh0 = dm2[0] * pw, dh1 = dm2[1] * pw, dh3 = -(dm2[0] * hom[0] + dm2[1] * hom[1]) * pw * pw;
 #pragma unroll
     for (int r = 0; r < 3; r++) dm[r] += sP[r * 4] * dh0 + sP[r * 4 + 1] * dh1 + sP[r * 4 + 3] * dh3;
+    if (DEPTH) dm[2] += g2.z;
     if (USE_SH) {
       float d[3] = {p[0] - sCam[0], p[1] - sCam[1], p[2] - sCam[2]};
       const float inv = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
@@ -704,7 +711,18 @@ int launch_project_fwd(const View& v, int64_t n, const float* means, const float
   if (n == 0) return 0;
   const unsigned blocks = (unsigned)((n + PROJ_THREADS - 1) / PROJ_THREADS);
   ProfScope ps(K_PROJECT_FWD, st);
-  if (v.num_channels == 6 && v.cov3d)      // six colour channels (checked by the caller: colors only, no raw_params / gather / band)
+  if (v.log_depth) {      // LoG's depth pass generated for any colour source (checked by the caller: no band mode)
+    if (v.cov3d && colors)
+      project_fwd_kernel<false, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+    else if (v.cov3d)
+      project_fwd_kernel<true, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+    else if (colors && shs)
+      project_fwd_kernel<false, true, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+    else if (colors)
+      project_fwd_kernel<false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+    else
+      project_fwd_kernel<true, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+  } else if (v.num_channels == 6 && v.cov3d)      // six colour channels (checked by the caller: colors only, no raw_params / gather / band)
     project_fwd_kernel<false, false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
   else if (v.num_channels == 6)
     project_fwd_kernel<false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
@@ -733,7 +751,18 @@ int launch_project_bwd(const View& v, int64_t n, const float* means, const float
   if (n == 0) return 0;
   const unsigned blocks = (unsigned)((n + PROJ_THREADS - 1) / PROJ_THREADS);
   ProfScope ps(K_PROJECT_BWD, st);
-  if (v.num_channels == 6 && v.cov3d)
+  if (v.log_depth) {      // dcolors (N,3) / dshs as without the depth pass (checked by the caller: no band mode, no rows)
+    if (v.cov3d && !use_sh)
+      project_bwd_kernel<false, false, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+    else if (v.cov3d)
+      project_bwd_kernel<true, false, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+    else if (!use_sh && shs)
+      project_bwd_kernel<false, false, true, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+    else if (!use_sh)
+      project_bwd_kernel<false, false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+    else
+      project_bwd_kernel<true, false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+  } else if (v.num_channels == 6 && v.cov3d)
     project_bwd_kernel<false, false, false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
   else if (v.num_channels == 6)
     project_bwd_kernel<false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);

@@ -34,11 +34,12 @@ class GatheredParams(dict):
 
 class _RenderGathered(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means2D, settings, tables, index, sh_degree_tables, filter_mode, params):
+    def forward(ctx, means2D, settings, tables, index, sh_degree_tables, filter_mode, params, log_depth=False):
         colors, shs = tables['colors'], tables.get('shs')
         use_shs = shs is not None and settings.sh_degree > 0
         out = rasterize_forward(settings, tables['xyz'], tables['opacity'].reshape(-1), tables['scaling'], tables['rotation'],
-                                colors, shs if use_shs else None, filter_mode, True, raw_params=True, gather_index=index)
+                                colors, shs if use_shs else None, filter_mode, True, raw_params=True, gather_index=index,
+                                log_depth=log_depth)
         image, radii, pid, pwp, pw, state = out
         state.image = None
         ctx.state, ctx.tables, ctx.params, ctx.use_shs = state, tables, params, use_shs
@@ -53,16 +54,17 @@ class _RenderGathered(torch.autograd.Function):
         ctx.state.image = image
         dm3, dm2, dop, dsc, drot, dcol, dsh = rasterize_backward(ctx.state, grad_image, t['xyz'], t['opacity'].reshape(-1), t['scaling'],
                                                                  t['rotation'], t['colors'], t.get('shs') if ctx.use_shs else None)
+        ctx.state.image = None      # no cycle image -> grad_fn -> ctx -> state -> image (see rasterizer._RasterizeGaussians)
         p = ctx.params
         p['xyz'].grad, p['scaling'].grad, p['rotation'].grad = dm3, dsc, drot
         p['opacity'].grad, p['colors'].grad = dop.reshape(-1, 1), dcol
         if 'shs' in p:
             p['shs'].grad = dsh
-        return dm2, None, None, None, None, None, None
+        return dm2, None, None, None, None, None, None, None
 
 
 def render_gathered(settings, tables: Dict[str, torch.Tensor], index: torch.Tensor, means2D: torch.Tensor, use_filter: bool = True,
-                    params: Optional[GatheredParams] = None):
+                    params: Optional[GatheredParams] = None, render_depth: bool = False):
     """Render rows `index` of LoG's raw parameter tables.
 
     tables : {'xyz' (N,3), 'scaling' (N,3) log-scales, 'rotation' (N,4) unnormalised, 'opacity' (N,1) logits,
@@ -71,9 +73,14 @@ def render_gathered(settings, tables: Dict[str, torch.Tensor], index: torch.Tens
     means2D: (M,3) zeros with requires_grad, LoG's `screenspace_points`; receives d loss / d (NDC x, y).
     Returns ((image, radii, point_id_pixel, point_weight_pixel, point_weight), point_count, params): the fork's 5-tuple
     for the M rendered rows, the winner histogram, and the GatheredParams whose `.grad` fields `loss.backward()` fills with
-    the compact raw-parameter gradients (same row order as `index`)."""
+    the compact raw-parameter gradients (same row order as `index`).
+    render_depth=True: LoG's depth pass in the same call; the image is (6,H,W), channels 3..5 being LoG's depth, height
+    and accmap (the colours (view depth, world z, 1) of the gathered means over settings.bg[:3]), and the height's
+    gradient lands in params['xyz'].grad.  With use_filter=False the depth channels are composited without the filter
+    too, which is not LoG's evaluation pair (colour without the filter, depth with it)."""
     if params is None:
         params = GatheredParams([k for k in ('xyz', 'scaling', 'rotation', 'opacity', 'colors', 'shs') if k in tables])
     tabs = {k: v.detach() for k, v in tables.items()}
-    out = _RenderGathered.apply(means2D, settings, tabs, index, None, LGR_FILTER_MAX if use_filter else LGR_FILTER_NONE, params)
+    out = _RenderGathered.apply(means2D, settings, tabs, index, None, LGR_FILTER_MAX if use_filter else LGR_FILTER_NONE, params,
+                                bool(render_depth))
     return out[:5], out[5], params

@@ -77,7 +77,8 @@ def _stream(device=None):
 
 def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: bool, sh_coeffs: int, tile_rows, keep,
                num_owners=0, band_ids=None, band_count=None, band_blk=None, band_rows=None, band_dsplat=None,
-               raw_params=False, tile_rank=None, gather_index=None, pid_map=None, cov3D_precomp=None, splat_ext=None):
+               raw_params=False, tile_rank=None, gather_index=None, pid_map=None, cov3D_precomp=None, splat_ext=None,
+               log_depth=False):
     dev = s.viewmatrix.device
     vm, pm = _f32c(s.viewmatrix, 'viewmatrix'), _f32c(s.projmatrix, 'projmatrix', dev)
     bg = _f32c(s.bg, 'bg', dev)
@@ -103,6 +104,7 @@ def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: boo
     v.cov3D_precomp_d = cov3D_precomp.data_ptr() if cov3D_precomp is not None else None
     if splat_ext is not None:      # six colour channels: channels 3..5 of every projected record live in splat_ext (N,4)
         v.num_channels, v.splat_ext_d = 6, splat_ext.data_ptr()
+        v.log_depth = int(bool(log_depth))      # ... generated by the projection as LoG's (view depth, world z, 1)
     v.viewmatrix_d, v.projmatrix_d = vm.data_ptr(), pm.data_ptr()
     v.campos_d = cp.data_ptr() if cp is not None else None
     v.bg_d = bg.data_ptr()
@@ -121,16 +123,23 @@ def set_contrib_lists(view, buf, D, n_contrib):
     view.last_contrib_d = n_contrib.data_ptr()
 
 
-def colour_channels(colors_precomp, settings, shs=None, raw_params=False, gather_index=None, num_owners=0):
-    """Number of precomputed colour channels of a call: 3, or 6 for colors_precomp (N,6), which composites six channels in
-    one pass (e.g. LoG's colour and its (depth, height, 1) pass).  Raises for any other width and for the combinations
-    six channels do not support."""
-    if colors_precomp is None:
-        return 3
-    width = int(colors_precomp.shape[-1]) if colors_precomp.dim() > 0 else 0
-    if width not in (3, 6):
-        raise _capi.LgrError(f'colors_precomp must have 3 or 6 channels per Gaussian, got shape {tuple(colors_precomp.shape)}')
-    if width == 3:
+def colour_channels(colors_precomp, settings, shs=None, raw_params=False, gather_index=None, num_owners=0, log_depth=False):
+    """Number of colour channels of a call's image: 3, or 6 for colors_precomp (N,6), which composites six channels in
+    one pass (e.g. LoG's colour and its (depth, height, 1) pass), and 6 with log_depth, where the projection generates
+    channels 3..5 for any colour source.  Raises for any other width and for the combinations six channels do not support."""
+    width = None
+    if colors_precomp is not None:
+        width = int(colors_precomp.shape[-1]) if colors_precomp.dim() > 0 else 0
+        if width not in (3, 6):
+            raise _capi.LgrError(f'colors_precomp must have 3 or 6 channels per Gaussian, got shape {tuple(colors_precomp.shape)}')
+    if log_depth:
+        if width == 6:
+            raise _capi.LgrError('render_depth generates the depth channels itself: pass three-channel colors_precomp (N,3), '
+                                 'not (N,6)')
+        if num_owners > 0:
+            raise _capi.LgrError('render_depth is not available in band mode (num_owners > 0)')
+        return 6
+    if width is None or width == 3:
         return 3
     if colors_precomp.dim() != 2:
         raise _capi.LgrError(f'six-channel colors_precomp must be (N,6), got shape {tuple(colors_precomp.shape)}')
@@ -154,7 +163,7 @@ class RasterState:
     __slots__ = ('view', 'keep', 'n', 'num_instances', 'max_tile_len', 'stock_instances', 'num_visible', 'splat',
                  'radii', 'clamped', 'tile_start', 'sorted_ids', 'final_T', 'n_contrib', 'image', 'sh', 'num_owners',
                  'band_ids', 'band_count', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D', 'contrib',
-                 'channels', 'splat_ext')
+                 'channels', 'splat_ext', 'log_depth')
 
     def read_stats(self):
         """Counters of this forward, read back from meta_d (synchronises): D, longest tile list, D by the stock rule, visible
@@ -175,7 +184,7 @@ class RasterState:
 
 def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_precomp, shs, filter_mode, want_aux,
                       tile_rows=None, num_owners=0, raw_params=False, prezero_dsplat=None, gather_index=None,
-                      instance_capacity=None, cov3D_precomp=None):
+                      instance_capacity=None, cov3D_precomp=None, log_depth=False):
     """Run the forward through the C ABI.  Returns (image, radii, pid, pwp, point_weight, state).
     num_owners > 0 (multi-GPU band mode, see log_b200/sharded.py): also compact the ids of the Gaussians reaching the
     band `tile_rows`, grouped by owner rank; the backward then returns packed gradient rows instead of dense tensors.
@@ -186,8 +195,16 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     cov3D_precomp (N,6): the stock API's precomputed world-space covariance (xx xy xz yy yz zz) instead of scales / rotations
     (pass those as None); the backward then returns its gradient in state.dcov3D.
     colors_precomp (N,6) with a 6-entry settings.bg: six channels composited in one pass, image (6,H,W); channels 0..2 equal a
-    call with colors_precomp[:, :3] and bg[:3] bit for bit, channels 3..5 one with [:, 3:] and bg[3:]."""
-    channels = colour_channels(colors_precomp, settings, shs, raw_params, gather_index, num_owners)
+    call with colors_precomp[:, :3] and bg[:3] bit for bit, channels 3..5 one with [:, 3:] and bg[3:].
+    log_depth=True: LoG's depth pass (renderer.py:186-201) in the same call, for any colour source above.  The image is
+    (6,H,W): channels 0..2 equal the call without log_depth bit for bit, channels 3..5 are LoG's depth, height and accmap,
+    i.e. the colours (view depth of the mean, world z of the mean, 1) composited over bg[:3].  colors_precomp stays (N,3)
+    (or None with shs) and so does its gradient; the height's gradient goes to means3D z, the depth's is dropped (LoG
+    computes it from the detached mean).  Not available in band mode."""
+    channels = colour_channels(colors_precomp, settings, shs, raw_params, gather_index, num_owners, log_depth)
+    if log_depth:      # the blend composites channels 3..5 over bg[3:6]: LoG's second call uses the same background
+        bg3 = settings.bg.reshape(-1)[:3]
+        settings = settings._replace(bg=torch.cat([bg3, bg3]))
     lib = _capi.load()
     dev = means3D.device
     if cov3D_precomp is not None and (raw_params or num_owners > 0):
@@ -225,10 +242,10 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         band_count = torch.empty((num_owners,), dtype=torch.int32, device=dev)
     tile_rank = torch.empty((max(n, 1), 4), dtype=torch.int32, device=dev) if RANKED_BIN else None
     keep.append(tile_rank)
-    splat_ext = torch.empty((n, 4), dtype=torch.float32, device=dev) if channels == 6 else None
+    splat_ext = torch.empty((max(n, 1), 4), dtype=torch.float32, device=dev) if channels == 6 else None      # never NULL
     keep.append(splat_ext)
     view = _make_view(settings, filter_mode, want_aux, K, tile_rows, keep, num_owners, band_ids, band_count, band_blk, band_rows, band_dsplat,
-                      raw_params, tile_rank, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext)
+                      raw_params, tile_rank, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext, log_depth=log_depth)
     H, W = view.image_height, view.image_width
     gx, gy = (W + 15) // 16, (H + 15) // 16
     rows = gy if tile_rows is None else int(tile_rows[1]) - int(tile_rows[0])
@@ -299,7 +316,7 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     s.final_T, s.n_contrib, s.image, s.sh = final_T, n_contrib, image, shs is not None
     s.point_count = pc
     s.contrib = contrib
-    s.channels, s.splat_ext = channels, splat_ext
+    s.channels, s.splat_ext, s.log_depth = channels, splat_ext, bool(log_depth)
     s.num_owners, s.band_ids, s.band_count = num_owners, (band_ids, band_blk, band_rows, band_dsplat), band_count
     s.band_counts_host = [int(x) for x in m[_capi.LGR_META_INTS:]] if num_owners > 0 else None
     return image, radii, pid, pwp, pw, s
@@ -345,7 +362,7 @@ def rasterize_backward(state: RasterState, grad_image, means3D, opacities, scale
     if cov:      # stock cov3D_precomp: the covariance gradient replaces the scale / rotation gradients
         state.dcov3D = torch.empty((n, 6), **f32)
         state.view.dcov3D_d = state.dcov3D.data_ptr()
-    dcolors = torch.empty((n, state.channels), **f32) if colors_precomp is not None else None
+    dcolors = torch.empty((n, 3 if state.log_depth else state.channels), **f32) if colors_precomp is not None else None
     dshs = torch.empty((n,) + tuple(shs.shape[1:]), **f32) if shs is not None else None
     _capi.check(lib.lgr_backward(ctypes.byref(state.view), n, state.num_instances, _ptr(means3D), _ptr(opacities),
                                  _ptr(scales), _ptr(rotations), _ptr(colors_precomp), _ptr(shs), _ptr(state.splat),
@@ -378,7 +395,8 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacities, colors_precomp, shs, scales, rotations, settings, filter_mode, want_aux,
-                tile_rows, raw_params=False, prezero_dsplat=False, instance_capacity=None, holder=None, cov3D_precomp=None):
+                tile_rows, raw_params=False, prezero_dsplat=False, instance_capacity=None, holder=None, cov3D_precomp=None,
+                log_depth=False):
         dev = means3D.device
         m = _f32c(means3D, 'means3D')
         o = _f32c(opacities, 'opacities', dev)
@@ -389,7 +407,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         sh = _f32c(shs, 'shs', dev)
         image, radii, pid, pwp, pw, state = rasterize_forward(settings, m, o, sc, r, c, sh, filter_mode, want_aux, tile_rows,
                                                               raw_params=raw_params, prezero_dsplat=prezero_dsplat,
-                                                              instance_capacity=instance_capacity, cov3D_precomp=cov)
+                                                              instance_capacity=instance_capacity, cov3D_precomp=cov,
+                                                              log_depth=log_depth)
         if holder is not None:
             holder['state'] = state
         state.image = None          # the backward re-reads the rendered image: saved below so autograd guards it
@@ -416,10 +435,13 @@ class _RasterizeGaussians(torch.autograd.Function):
             ctx.state.cov3D = cov
         ctx.state.image = image
         dm3, dm2, dop, dsc, drot, dcol, dsh = rasterize_backward(ctx.state, grad_image, m, o, sc, r, c, sh)
+        # the unpacked image's grad_fn is this node: a reference kept in the state would make a cycle that holds the graph
+        # and every tensor it reaches until the garbage collector runs
+        ctx.state.image = None
         if ctx.debug and m.is_cuda:
             torch.cuda.synchronize(m.device)
         return (dm3, dm2, dop.reshape(ctx.opacity_shape), dcol, dsh, dsc, drot, None, None, None, None, None, None, None, None,
-                ctx.state.dcov3D)
+                ctx.state.dcov3D, None)
 
 
 class GaussianRasterizer(nn.Module):
@@ -451,7 +473,14 @@ class GaussianRasterizer(nn.Module):
                               s.image_width / (2.0 * s.tanfovx), s.image_height / (2.0 * s.tanfovy), s.tanfovx, s.tanfovy)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, use_filter=True, raw_params=False):
+                cov3D_precomp=None, use_filter=True, raw_params=False, render_depth=False):
+        """render_depth=True: LoG's depth pass (renderer.py:186-201) in the same call.  The image is (6,H,W): channels 0..2
+        are the colour image of the call without render_depth, bit for bit; channels 3..5 are LoG's depth, height and
+        accmap, the colours (view depth of the mean, world z of the mean, 1) composited over raster_settings.bg[:3] with the
+        same Gaussians and settings.  Any colour source works (colors_precomp (N,3), shs, raw_params); colors_precomp
+        (N,6) raises.  The height's gradient goes to means3D z; the depth's is dropped, as LoG detaches it.  With
+        use_filter=False both halves are composited without the filter: that is not LoG's evaluation pair, which renders
+        the colour without the filter and the depth with it (two calls)."""
         log_sh = raw_params and shs is not None and colors_precomp is not None      # LoG's colour activation fused
         if (shs is None) == (colors_precomp is None) and not log_sh:
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
@@ -474,7 +503,8 @@ class GaussianRasterizer(nn.Module):
         holder = {}
         out = _RasterizeGaussians.apply(means3D, means2D, opacities, colors_precomp, shs, scales, rotations,
                                         self.raster_settings, filter_mode, fork, self.tile_rows, raw_params,
-                                        PREZERO_DSPLAT and needs_grad, self.instance_capacity, holder, cov3D_precomp)
+                                        PREZERO_DSPLAT and needs_grad, self.instance_capacity, holder, cov3D_precomp,
+                                        bool(render_depth))
         self.last_state = holder.get('state')
         if self.raster_settings.debug and means3D.is_cuda:      # stock `debug`: surface a kernel fault at the call that caused it
             torch.cuda.synchronize(means3D.device)

@@ -268,12 +268,14 @@ class SplatExchange:
 
     # ---- phases (forward() / backward() below string them together with the barriers) --------------------------
     def project_and_send(self, settings, means3D, opacities, scales, rotations, colors_precomp=None, shs=None,
-                         filter_mode=None, want_aux=True, raw_params=False) -> ShardStep:
+                         filter_mode=None, want_aux=True, raw_params=False, render_depth=False) -> ShardStep:
         """Project this rank's shard (inputs are the LOCAL rows [lo,hi) of the model) and push the visible records."""
         import ctypes
         from . import _capi
         from .rasterizer import _f32c, _make_view, _ptr, _stream
         lib = _capi.load()
+        if render_depth:
+            raise _capi.LgrError('render_depth is not available in shard mode: the exchange moves three-channel records only')
         if colors_precomp is not None and int(colors_precomp.shape[-1]) != 3:
             raise _capi.LgrError(f'shard mode renders three precomputed colour channels, got colors_precomp {tuple(colors_precomp.shape)}')
         filter_mode = _capi.LGR_FILTER_MAX if filter_mode is None else filter_mode
