@@ -8,11 +8,11 @@ namespace lgr {
 int launch_mark_visible(int64_t, const float*, const float*, uint8_t*, cudaStream_t);
 int launch_compute_radius(int64_t, const float*, const float*, const float*, const float*, const float*, float, float,
                           float, float, float*, cudaStream_t);
-int launch_project_fwd(const View&, int64_t, const float*, const float*, const float*, const float*, const float*,
-                       const float*, float*, int32_t*, uint8_t*, int32_t*, int32_t*, cudaStream_t);
-int launch_project_bwd(const View&, int64_t, const float*, const float*, const float*, const float*, const float*, bool,
-                       const int32_t*, const uint8_t*, const float*, float*, float*, float*, float*, float*, float*,
-                       float*, float*, void* const*, int, cudaStream_t);
+int launch_project_fwd(const View&, Colour, bool, int64_t, const float*, const float*, const float*, const float*,
+                       const float*, const float*, float*, int32_t*, uint8_t*, int32_t*, int32_t*, cudaStream_t);
+int launch_project_bwd(const View&, Colour, bool, bool, int64_t, const float*, const float*, const float*, const float*,
+                       const float*, const int32_t*, const uint8_t*, const float*, float*, float*, float*, float*, float*,
+                       float*, float*, float*, void* const*, int, cudaStream_t);
 int launch_grad_scatter_add(int64_t, const float*, int64_t, int64_t, float*, cudaStream_t);
 int launch_grad_scatter_add_staged(const float*, int, int64_t, int64_t, int64_t, float*, cudaStream_t);
 int launch_band_scan(const View&, cudaStream_t);
@@ -68,6 +68,18 @@ static int six_channels_check(const lgr_view* v) {
   return 0;
 }
 
+// The colour source of a projection call: colors_precomp XOR shs (stock), colors_precomp (N,6) with six channels unless
+// the projection generates channels 3..5 (log_depth), or -- with raw_params -- LoG's raw DC colours + the rest
+// coefficients (LoG's colour activation fused, activation.py:27-34).  0 when the pair of tables names one.
+static int colour_source(const lgr_view* v, int64_t n, const float* colors_precomp_d, const float* shs_d, Colour* c) {
+  const bool six_precomp = v->num_channels == 6 && !v->log_depth;
+  if (six_precomp && shs_d) return LGR_E_UNSUPPORTED;
+  const bool log_sh = v->raw_params && colors_precomp_d && shs_d;
+  if (!log_sh && (colors_precomp_d != nullptr) == (shs_d != nullptr) && n > 0) return LGR_E_BADARG;
+  *c = log_sh ? Colour::LOG_SH : shs_d ? Colour::SH : six_precomp ? Colour::RGB6 : Colour::RGB;
+  return 0;
+}
+
 extern "C" {
 
 int lgr_abi_version(void) { return LGR_ABI_VERSION; }
@@ -94,20 +106,15 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
                         int32_t* tile_start_d, int32_t* tile_cursor_d, int32_t* meta_d, void* stream) {
   if (!view_ok(view) || n < 0 || !tile_start_d || !tile_cursor_d || !meta_d) return LGR_E_BADARG;
   if (const int rc6 = six_channels_check(view)) return rc6;
-  const bool six_precomp = view->num_channels == 6 && !view->log_depth;      // colors_precomp (N,6)
-  if (six_precomp && shs_d) return LGR_E_UNSUPPORTED;
-  if (six_precomp && n > 0 && !colors_precomp_d) return LGR_E_BADARG;
-  // colour sources: colors_precomp XOR shs (stock), or -- with raw_params -- raw DC colours + the rest coefficients
-  // (LoG's colour activation fused, activation.py:27-34)
-  const bool log_sh = view->raw_params && colors_precomp_d && shs_d;
-  if (!log_sh && (colors_precomp_d != nullptr) == (shs_d != nullptr) && n > 0) return LGR_E_BADARG;
-  if (view->raw_params && shs_d && !colors_precomp_d) return LGR_E_UNSUPPORTED;   // raw stock-layout SH is not a LoG input
-  if (log_sh) {
+  Colour c;
+  if (const int rc = colour_source(view, n, colors_precomp_d, shs_d, &c)) return rc;
+  if (view->raw_params && c == Colour::SH) return LGR_E_UNSUPPORTED;   // raw stock-layout SH is not a LoG input
+  if (c == Colour::LOG_SH) {
     if (!view->campos_d) return LGR_E_BADARG;
     if (view->sh_degree < 0 || view->sh_degree > 3) return LGR_E_UNSUPPORTED;
     if (view->sh_coeffs < (view->sh_degree + 1) * (view->sh_degree + 1) - 1) return LGR_E_BADARG;
     if (view->num_owners > 0) return LGR_E_UNSUPPORTED;
-  } else if (shs_d) {
+  } else if (c == Colour::SH) {
     if (!view->campos_d || !clamped_d) return LGR_E_BADARG;
     if (view->sh_degree < 0 || view->sh_degree > 3) return LGR_E_UNSUPPORTED;
     if (view->sh_coeffs < (view->sh_degree + 1) * (view->sh_degree + 1)) return LGR_E_BADARG;
@@ -119,15 +126,13 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
   cudaStream_t st = (cudaStream_t)stream;
   const View v = make_view(view, n);
   const int ntiles = v.gx * (v.row1 - v.row0);
-  if (v.num_owners > 0) {
-    if (shs_d) return LGR_E_UNSUPPORTED;          // band mode packs 17-float rows: precomputed colours only
-  }
-  if (log_sh && view->sh_degree == 0) shs_d = nullptr;      // degree 0: the rest coefficients are not read
+  if (v.num_owners > 0 && shs_d) return LGR_E_UNSUPPORTED;      // band mode packs 17-float rows: precomputed colours only
+  if (c == Colour::LOG_SH && view->sh_degree == 0) c = Colour::RGB;      // degree 0: the rest coefficients are not read
   cudaError_t e = cudaMemsetAsync(tile_cursor_d, 0, sizeof(int32_t) * (size_t)ntiles * CSTRIDE, st);
   if (e != cudaSuccess) return (int)e;
   e = cudaMemsetAsync(meta_d, 0, sizeof(int32_t) * LGR_META_INTS, st);
   if (e != cudaSuccess) return (int)e;
-  int rc = launch_project_fwd(v, n, means3D_d, opacities_d, scales_d, rotations_d, colors_precomp_d, shs_d, splat_d,
+  int rc = launch_project_fwd(v, c, cov3d, n, means3D_d, opacities_d, scales_d, rotations_d, colors_precomp_d, shs_d, splat_d,
                               radii_d, clamped_d, tile_cursor_d, meta_d, st);
   if (rc) return rc;
   rc = launch_band_scan(v, st);
@@ -192,24 +197,24 @@ int lgr_backward(const lgr_view* view, int64_t n, int64_t num_instances, const f
                  int64_t num_rows, void* stream) {
   if (!view_ok(view) || n < 0 || !tile_start_d || !image_d || !dL_dimage_d) return LGR_E_BADARG;
   if (const int rc6 = six_channels_check(view)) return rc6;
-  if (view->num_channels == 6 && ((shs_d && !view->log_depth) || grad_rows_d || peer_stage_d)) return LGR_E_UNSUPPORTED;
+  const bool rows_mode = grad_rows_d || peer_stage_d;
+  if (view->num_channels == 6 && rows_mode) return LGR_E_UNSUPPORTED;
+  Colour c;
+  if (const int rc = colour_source(view, n, colors_precomp_d, shs_d, &c)) return rc;
   if (n == 0) return 0;
-  const bool log_sh = view->raw_params && colors_precomp_d && shs_d;      // LoG-style SH: DC colours + rest coefficients
-  const bool use_sh = shs_d != nullptr && !log_sh;
-  if (!log_sh && use_sh == (colors_precomp_d != nullptr)) return LGR_E_BADARG;
-  if (log_sh && (!dshs_d || !view->campos_d || view->num_owners > 0)) return LGR_E_BADARG;
+  if (c == Colour::LOG_SH && (!dshs_d || !view->campos_d || view->num_owners > 0)) return LGR_E_BADARG;
   const bool cov3d = view->cov3D_precomp_d != nullptr;
   if (!means3D_d || (!cov3d && (!scales_d || !rotations_d)) || !splat_d || !radii_d || !dsplat_d) return LGR_E_BADARG;
   if (cov3d && (!view->dcov3D_d || view->raw_params || view->num_owners > 0 || grad_rows_d || peer_stage_d)) return LGR_E_BADARG;
-  if (view->raw_params && (!opacities_d || use_sh)) return LGR_E_BADARG;
-  if (grad_rows_d || peer_stage_d) {
-    if (view->num_owners <= 0 || use_sh) return LGR_E_BADARG;
+  if (view->raw_params && (!opacities_d || c == Colour::SH)) return LGR_E_BADARG;
+  if (rows_mode) {
+    if (view->num_owners <= 0 || c == Colour::SH) return LGR_E_BADARG;
     if (peer_stage_d && (my_rank < 0 || my_rank >= view->num_owners)) return LGR_E_BADARG;
     if (num_rows < 0 || num_rows > n) return LGR_E_BADARG;
   } else {
     if (view->num_owners > 0) return LGR_E_BADARG;   // band mode writes no splat records outside the band: rows only
     if (!dmeans3D_d || !dmeans2D_d || !dopacities_d || (!cov3d && (!dscales_d || !drotations_d))) return LGR_E_BADARG;
-    if (use_sh ? (!dshs_d || !clamped_d || !view->campos_d) : !dcolors_d) return LGR_E_BADARG;
+    if (c == Colour::SH ? (!dshs_d || !clamped_d || !view->campos_d) : !dcolors_d) return LGR_E_BADARG;
   }
   if (num_instances > 0 && !sorted_ids_d) return LGR_E_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
@@ -217,8 +222,7 @@ int lgr_backward(const lgr_view* view, int64_t n, int64_t num_instances, const f
   int rc = 0;
   if (num_instances > 0) rc = launch_blend_bwd(v, tile_start_d, sorted_ids_d, splat_d, image_d, dL_dimage_d, dsplat_d, st);
   if (rc) return rc;
-  const bool rows_mode = grad_rows_d || peer_stage_d;
-  return launch_project_bwd(v, rows_mode ? num_rows : n, means3D_d, opacities_d, scales_d, rotations_d, (use_sh || log_sh) ? shs_d : nullptr, use_sh, radii_d, clamped_d, dsplat_d,
+  return launch_project_bwd(v, c, cov3d, rows_mode, rows_mode ? num_rows : n, means3D_d, opacities_d, scales_d, rotations_d, shs_d, radii_d, clamped_d, dsplat_d,
                             dmeans3D_d, dmeans2D_d, dopacities_d, dscales_d, drotations_d, dcolors_d, dshs_d, grad_rows_d, peer_stage_d, my_rank, st);
 }
 

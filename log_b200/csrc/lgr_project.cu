@@ -15,6 +15,29 @@ __device__ __forceinline__ void load3(const float* __restrict__ p, int64_t i, fl
   o[0] = __ldg(p + 3 * i); o[1] = __ldg(p + 3 * i + 1); o[2] = __ldg(p + 3 * i + 2);
 }
 
+// stock cov3D_precomp, row i: upper triangle xx xy xz yy yz zz, used as given (no scale modifier, like the stock rasteriser)
+__device__ __forceinline__ void load_cov3d(const float* cov, int64_t i, float Sg[9]) {
+  const float* c6 = cov + 6 * i;
+  const float cxx = __ldg(c6), cxy = __ldg(c6 + 1), cxz = __ldg(c6 + 2), cyy = __ldg(c6 + 3), cyz = __ldg(c6 + 4), czz = __ldg(c6 + 5);
+  Sg[0] = cxx; Sg[1] = cxy; Sg[2] = cxz; Sg[3] = cxy; Sg[4] = cyy; Sg[5] = cyz; Sg[6] = cxz; Sg[7] = cyz; Sg[8] = czz;
+}
+
+// the SH basis at the unit view direction from the camera to p
+__device__ __forceinline__ void sh_dir_basis(const float p[3], const float* cam, int deg, float B[16]) {
+  const float d[3] = {p[0] - cam[0], p[1] - cam[1], p[2] - cam[2]};
+  const float inv = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+  sh_basis(deg, d[0] * inv, d[1] * inv, d[2] * inv, B);
+}
+
+// The two SH layouts: stock (first = 0) holds coefficients 0 .. nb-1 of a row, LoG's rest (first = 1) holds 1 .. nb-1.
+// rgb += sum_k B_k sh_k
+__device__ __forceinline__ void sh_accumulate(const float* sh, const float B[16], int first, int nb, float rgb[3]) {
+  for (int k = first; k < nb; k++) {
+    rgb[0] += B[k] * __ldg(sh + 3 * (k - first)); rgb[1] += B[k] * __ldg(sh + 3 * (k - first) + 1);
+    rgb[2] += B[k] * __ldg(sh + 3 * (k - first) + 2);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // markVisible of the stock module (diff_gaussian_rasterization's GaussianRasterizer.markVisible): a point is visible
 // when its view-space depth exceeds the near plane -- the same cull the projection applies (NEAR_Z)
@@ -55,21 +78,24 @@ compute_radius_kernel(int64_t n, const float* __restrict__ means, const float* _
 // ---------------------------------------------------------------------------------------------------------
 // forward projection
 // ---------------------------------------------------------------------------------------------------------
-// LOG_SH (with USE_SH = false and View::raw_params): LoG's colour activation (LoG/model/activation.py:27-34) fused --
+// C = LOG_SH (View::raw_params): LoG's colour activation (LoG/model/activation.py:27-34) fused --
 // rgb = SH2RGB(dc) + eval_sh_wobase(dir, rest, degree) with dc = `colors` (N,3) raw and rest = `shs` (N,K,3); unlike the
 // stock SH path there is NO clamp at 0 and the direction comes from the DETACHED position (no gradient to the mean).
 // COV3D: the world-space covariance comes precomputed from View::cov3d (stock cov3D_precomp) instead of scales / rotations.
-// SIX: six precomputed colour channels, `colors` (N,6); channels 3..5 go to View::splat_ext (N,4) as (c3, c4, c5, 0).
+// C = RGB6: six precomputed colour channels, `colors` (N,6); channels 3..5 go to View::splat_ext (N,4) as (c3, c4, c5, 0).
 // DEPTH (View::log_depth): channels 3..5 are LoG's depth-pass colours (renderer.py:186-201), generated here for any colour
 // source: (view depth, world z, 1) -> View::splat_ext as (t_z, p_z, 1, 0); t_z is the unclamped view-space z of the mean
 // (cov2d's t[2], record float 11).
-template <bool USE_SH, bool LOG_SH = false, bool COV3D = false, bool SIX = false, bool DEPTH = false>
+template <Colour C, bool COV3D, bool DEPTH>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
                    const float* __restrict__ scales, const float* __restrict__ rots,
                    const float* __restrict__ colors, const float* __restrict__ shs, float* __restrict__ splat,
                    int32_t* __restrict__ radii, uint8_t* __restrict__ clamped, int32_t* __restrict__ tile_count,
                    int32_t* __restrict__ meta) {
+  static_assert(!(C == Colour::RGB6 && DEPTH), "the depth pass generates channels 3..5: colours are (N,3)");
+  static_assert(!(C == Colour::LOG_SH && COV3D), "LoG's raw parameters come with scales and rotations");
+  constexpr bool USE_SH = C == Colour::SH, LOG_SH = C == Colour::LOG_SH, SIX = C == Colour::RGB6;
   __shared__ float sV[16], sP[16], sCam[3];
   __shared__ float sWf;
   __shared__ unsigned sStock[PROJ_THREADS / 32];
@@ -146,10 +172,8 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
   if (work) {
     float p[3], Sg[9];
     load3(means, src, p);
-    if (COV3D) {      // upper triangle xx xy xz yy yz zz, used as given (no scale modifier, like the stock rasteriser)
-      const float* c6 = v.cov3d + 6 * src;
-      const float cxx = __ldg(c6), cxy = __ldg(c6 + 1), cxz = __ldg(c6 + 2), cyy = __ldg(c6 + 3), cyz = __ldg(c6 + 4), czz = __ldg(c6 + 5);
-      Sg[0] = cxx; Sg[1] = cxy; Sg[2] = cxz; Sg[3] = cxy; Sg[4] = cyy; Sg[5] = cyz; Sg[6] = cxz; Sg[7] = cyz; Sg[8] = czz;
+    if (COV3D) {
+      load_cov3d(v.cov3d, src, Sg);
     } else {
       float s[3], R[9];
       load3(scales, src, s);
@@ -196,16 +220,10 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
         }
         float rgb[3];
         if (USE_SH) {
-          float d[3] = {p[0] - sCam[0], p[1] - sCam[1], p[2] - sCam[2]};
-          const float inv = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
           float B[16];
-          sh_basis(v.sh_degree, d[0] * inv, d[1] * inv, d[2] * inv, B);
-          const int nb = (v.sh_degree + 1) * (v.sh_degree + 1);
-          const float* sh = shs + src * v.sh_K * 3;
+          sh_dir_basis(p, sCam, v.sh_degree, B);
           rgb[0] = rgb[1] = rgb[2] = 0.5f;
-          for (int k = 0; k < nb; k++) {
-            rgb[0] += B[k] * __ldg(sh + 3 * k); rgb[1] += B[k] * __ldg(sh + 3 * k + 1); rgb[2] += B[k] * __ldg(sh + 3 * k + 2);
-          }
+          sh_accumulate(shs + src * v.sh_K * 3, B, 0, (v.sh_degree + 1) * (v.sh_degree + 1), rgb);
           uint8_t cl = 0;
 #pragma unroll
           for (int ch = 0; ch < 3; ch++) if (rgb[ch] < 0.0f) { cl |= (uint8_t)(1u << ch); rgb[ch] = 0.0f; }
@@ -221,16 +239,9 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
             for (int ch = 0; ch < 3; ch++) rgb[ch] = fmaf(SH_C0, rgb[ch], 0.5f);
           }
           if (LOG_SH && v.sh_degree > 0) {      // + eval_sh_wobase (sh_utils.py:31-58): basis functions 1 .. (deg+1)^2 - 1
-            float d[3] = {p[0] - sCam[0], p[1] - sCam[1], p[2] - sCam[2]};
-            const float inv = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
             float B[16];
-            sh_basis(v.sh_degree, d[0] * inv, d[1] * inv, d[2] * inv, B);
-            const int nb = (v.sh_degree + 1) * (v.sh_degree + 1);
-            const float* sh = shs + src * v.sh_K * 3;
-            for (int k = 1; k < nb; k++) {
-              rgb[0] += B[k] * __ldg(sh + 3 * (k - 1)); rgb[1] += B[k] * __ldg(sh + 3 * (k - 1) + 1);
-              rgb[2] += B[k] * __ldg(sh + 3 * (k - 1) + 2);
-            }
+            sh_dir_basis(p, sCam, v.sh_degree, B);
+            sh_accumulate(shs + src * v.sh_K * 3, B, 1, (v.sh_degree + 1) * (v.sh_degree + 1), rgb);
           }
         }
         // conic pre-multiplied by log2(e): the blend evaluates alpha = o * 2^(-0.5 d^T C' d)
@@ -289,10 +300,11 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
 // ---------------------------------------------------------------------------------------------------------
 // backward projection: dsplat (d/dpx, d/dpy, d/dconic xyz, d/dopacity, d/drgb) -> input gradients
 // ---------------------------------------------------------------------------------------------------------
-// SIX: six precomputed colour channels; d/dc3..5 are floats 9..11 of the dsplat row, dcolors is (N,6).
+// C = RGB6: six precomputed colour channels; d/dc3..5 are floats 9..11 of the dsplat row, dcolors is (N,6).
 // DEPTH (View::log_depth): channels 3..5 were generated as (view depth, world z, 1).  d/dc4 (height = the mean's z) goes to
 // dmeans3D z; d/dc3 is dropped (LoG computes the depth from the detached mean) and so is d/dc5 (a constant).
-template <bool USE_SH, bool ROWS, bool LOG_SH = false, bool COV3D = false, bool SIX = false, bool DEPTH = false>
+// ROWS (band mode): one packed gradient row per listed Gaussian instead of the dense outputs.
+template <Colour C, bool COV3D, bool DEPTH, bool ROWS>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
                    const float* __restrict__ scales, const float* __restrict__ rots, const float* __restrict__ shs, const int32_t* __restrict__ radii,
@@ -300,6 +312,10 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
                    float* __restrict__ dmeans2D, float* __restrict__ dopac, float* __restrict__ dscales,
                    float* __restrict__ drots, float* __restrict__ dcolors, float* __restrict__ dshs,
                    float* __restrict__ grad_rows, void* const* __restrict__ peer_stage, int my_rank) {
+  static_assert(!(C == Colour::RGB6 && DEPTH), "the depth pass generates channels 3..5: colours are (N,3)");
+  static_assert(!(C == Colour::LOG_SH && COV3D), "LoG's raw parameters come with scales and rotations");
+  static_assert(!ROWS || (C == Colour::RGB && !COV3D && !DEPTH), "band mode rows carry three precomputed colours only");
+  constexpr bool USE_SH = C == Colour::SH, LOG_SH = C == Colour::LOG_SH, SIX = C == Colour::RGB6;
   __shared__ float sV[16], sP[16], sCam[3];
   if (threadIdx.x < 16) { sV[threadIdx.x] = v.view[threadIdx.x]; sP[threadIdx.x] = v.proj[threadIdx.x]; }
   if ((USE_SH || LOG_SH) && threadIdx.x < 3) sCam[threadIdx.x] = v.campos[threadIdx.x];
@@ -335,9 +351,7 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
     float q_inv = 1.0f;
     if (COV3D) {
-      const float* c6 = v.cov3d + 6 * src;
-      const float cxx = __ldg(c6), cxy = __ldg(c6 + 1), cxz = __ldg(c6 + 2), cyy = __ldg(c6 + 3), cyz = __ldg(c6 + 4), czz = __ldg(c6 + 5);
-      Sg[0] = cxx; Sg[1] = cxy; Sg[2] = cxz; Sg[3] = cxy; Sg[4] = cyy; Sg[5] = cyz; Sg[6] = cxz; Sg[7] = cyz; Sg[8] = czz;
+      load_cov3d(v.cov3d, src, Sg);
     } else {
       load3(scales, src, s0);
       q = ldg4(rots + 4 * src);
@@ -502,12 +516,9 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
       float* dsh = dshs + (int64_t)i * K * 3;
       int nb = 1;
       if (v.sh_degree > 0) {
-        float p[3];
+        float p[3], B[16];
         load3(means, src, p);
-        const float d[3] = {p[0] - sCam[0], p[1] - sCam[1], p[2] - sCam[2]};
-        const float inv_d = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-        float B[16];
-        sh_basis(v.sh_degree, d[0] * inv_d, d[1] * inv_d, d[2] * inv_d, B);
+        sh_dir_basis(p, sCam, v.sh_degree, B);
         nb = (v.sh_degree + 1) * (v.sh_degree + 1);
         for (int k = 1; k < nb; k++) {
           dsh[3 * (k - 1)] = B[k] * drgb[0]; dsh[3 * (k - 1) + 1] = B[k] * drgb[1]; dsh[3 * (k - 1) + 2] = B[k] * drgb[2];
@@ -705,79 +716,54 @@ int launch_mark_visible(int64_t n, const float* means, const float* view, uint8_
   return 0;
 }
 
-int launch_project_fwd(const View& v, int64_t n, const float* means, const float* opac, const float* scales,
-                       const float* rots, const float* colors, const float* shs, float* splat, int32_t* radii,
-                       uint8_t* clamped, int32_t* tile_count, int32_t* meta, cudaStream_t st) {
+// The projection kernels, by [colour source][cov3D_precomp][depth pass]; nullptr: no such call (lgr_capi.cu rejects it)
+using ProjectFwd = decltype(&project_fwd_kernel<Colour::RGB, false, false>);
+using ProjectBwd = decltype(&project_bwd_kernel<Colour::RGB, false, false, false>);
+static const ProjectFwd kProjectFwd[4][2][2] = {
+    {{project_fwd_kernel<Colour::RGB, false, false>, project_fwd_kernel<Colour::RGB, false, true>},
+     {project_fwd_kernel<Colour::RGB, true, false>, project_fwd_kernel<Colour::RGB, true, true>}},
+    {{project_fwd_kernel<Colour::SH, false, false>, project_fwd_kernel<Colour::SH, false, true>},
+     {project_fwd_kernel<Colour::SH, true, false>, project_fwd_kernel<Colour::SH, true, true>}},
+    {{project_fwd_kernel<Colour::LOG_SH, false, false>, project_fwd_kernel<Colour::LOG_SH, false, true>}, {nullptr, nullptr}},
+    {{project_fwd_kernel<Colour::RGB6, false, false>, nullptr}, {project_fwd_kernel<Colour::RGB6, true, false>, nullptr}}};
+static const ProjectBwd kProjectBwd[4][2][2] = {
+    {{project_bwd_kernel<Colour::RGB, false, false, false>, project_bwd_kernel<Colour::RGB, false, true, false>},
+     {project_bwd_kernel<Colour::RGB, true, false, false>, project_bwd_kernel<Colour::RGB, true, true, false>}},
+    {{project_bwd_kernel<Colour::SH, false, false, false>, project_bwd_kernel<Colour::SH, false, true, false>},
+     {project_bwd_kernel<Colour::SH, true, false, false>, project_bwd_kernel<Colour::SH, true, true, false>}},
+    {{project_bwd_kernel<Colour::LOG_SH, false, false, false>, project_bwd_kernel<Colour::LOG_SH, false, true, false>},
+     {nullptr, nullptr}},
+    {{project_bwd_kernel<Colour::RGB6, false, false, false>, nullptr}, {project_bwd_kernel<Colour::RGB6, true, false, false>, nullptr}}};
+
+int launch_project_fwd(const View& v, Colour c, bool cov3d, int64_t n, const float* means, const float* opac,
+                       const float* scales, const float* rots, const float* colors, const float* shs, float* splat,
+                       int32_t* radii, uint8_t* clamped, int32_t* tile_count, int32_t* meta, cudaStream_t st) {
   if (n == 0) return 0;
+  const ProjectFwd k = kProjectFwd[(int)c][cov3d][v.log_depth];
+  if (!k) return LGR_E_UNSUPPORTED;
   const unsigned blocks = (unsigned)((n + PROJ_THREADS - 1) / PROJ_THREADS);
   ProfScope ps(K_PROJECT_FWD, st);
-  if (v.log_depth) {      // LoG's depth pass generated for any colour source (checked by the caller: no band mode)
-    if (v.cov3d && colors)
-      project_fwd_kernel<false, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-    else if (v.cov3d)
-      project_fwd_kernel<true, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-    else if (colors && shs)
-      project_fwd_kernel<false, true, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-    else if (colors)
-      project_fwd_kernel<false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-    else
-      project_fwd_kernel<true, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  } else if (v.num_channels == 6 && v.cov3d)      // six colour channels (checked by the caller: colors only, no raw_params / gather / band)
-    project_fwd_kernel<false, false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  else if (v.num_channels == 6)
-    project_fwd_kernel<false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  else if (v.cov3d && colors)      // stock cov3D_precomp (checked by the caller: no raw_params, no band mode)
-    project_fwd_kernel<false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  else if (v.cov3d)
-    project_fwd_kernel<true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  else if (colors && shs)      // LoG-style SH on top of raw DC colours (checked by the caller: raw_params, no band mode)
-    project_fwd_kernel<false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  else if (colors)
-    project_fwd_kernel<false><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
-  else
-    project_fwd_kernel<true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
+  k<<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, colors, shs, splat, radii, clamped, tile_count, meta);
   LGR_CHECK_LAUNCH();
   return 0;
 }
 
-int launch_project_bwd(const View& v, int64_t n, const float* means, const float* opac, const float* scales, const float* rots,
-                       const float* shs, bool use_sh, const int32_t* radii, const uint8_t* clamped, const float* dsplat,
-                       float* dmeans, float* dmeans2D, float* dopac, float* dscales, float* drots, float* dcolors,
-                       float* dshs, float* grad_rows, void* const* peer_stage, int my_rank, cudaStream_t st) {
+// rows (band mode): one packed gradient row per listed Gaussian; precomputed (N,3) colours only (lgr_capi.cu)
+int launch_project_bwd(const View& v, Colour c, bool cov3d, bool rows, int64_t n, const float* means, const float* opac,
+                       const float* scales, const float* rots, const float* shs, const int32_t* radii, const uint8_t* clamped,
+                       const float* dsplat, float* dmeans, float* dmeans2D, float* dopac, float* dscales, float* drots,
+                       float* dcolors, float* dshs, float* grad_rows, void* const* peer_stage, int my_rank, cudaStream_t st) {
   if (peer_stage) {      // owners must learn this rank's row counts even when they are zero
     push_counts_kernel<<<1, 64, 0, st>>>(v, peer_stage, my_rank);
     LGR_CHECK_LAUNCH();
   }
   if (n == 0) return 0;
+  const ProjectBwd k = rows ? project_bwd_kernel<Colour::RGB, false, false, true> : kProjectBwd[(int)c][cov3d][v.log_depth];
+  if (!k) return LGR_E_UNSUPPORTED;
   const unsigned blocks = (unsigned)((n + PROJ_THREADS - 1) / PROJ_THREADS);
   ProfScope ps(K_PROJECT_BWD, st);
-  if (v.log_depth) {      // dcolors (N,3) / dshs as without the depth pass (checked by the caller: no band mode, no rows)
-    if (v.cov3d && !use_sh)
-      project_bwd_kernel<false, false, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-    else if (v.cov3d)
-      project_bwd_kernel<true, false, false, true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-    else if (!use_sh && shs)
-      project_bwd_kernel<false, false, true, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-    else if (!use_sh)
-      project_bwd_kernel<false, false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-    else
-      project_bwd_kernel<true, false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  } else if (v.num_channels == 6 && v.cov3d)
-    project_bwd_kernel<false, false, false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else if (v.num_channels == 6)
-    project_bwd_kernel<false, false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else if (v.cov3d && !use_sh)
-    project_bwd_kernel<false, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else if (v.cov3d)
-    project_bwd_kernel<true, false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else if (grad_rows || peer_stage)
-    project_bwd_kernel<false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else if (!use_sh && shs)      // LoG-style SH: dcolors (DC) and dshs (rest) both written
-    project_bwd_kernel<false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else if (!use_sh)
-    project_bwd_kernel<false, false><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
-  else
-    project_bwd_kernel<true, false><<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac, dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
+  k<<<blocks, PROJ_THREADS, 0, st>>>(v, n, means, opac, scales, rots, shs, radii, clamped, dsplat, dmeans, dmeans2D, dopac,
+                                     dscales, drots, dcolors, dshs, grad_rows, peer_stage, my_rank);
   LGR_CHECK_LAUNCH();
   return 0;
 }

@@ -1,9 +1,14 @@
 """SASS census of the shipped library: which tensor-core / matrix-load / warp-collective / atomic instructions each kernel
-contains.  python profiles/sass_census.py > census.md   (needs cuobjdump and c++filt; no GPU)"""
+contains.  python profiles/sass_census.py > census.md   (needs cuobjdump and c++filt; no GPU)
+
+python profiles/sass_census.py --bodies: one line per kernel -- a hash of its instruction text (addresses and encodings
+stripped), its instruction count and its demangled name -- to diff two builds and show which kernels a change recompiled."""
 import collections
+import hashlib
 import os
 import re
 import subprocess
+import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'log_b200', '_lib', 'liblog_b200_raster.so')
@@ -15,8 +20,27 @@ PATS = collections.OrderedDict([
     ('CCTL (L2 prefetch)', r'\bCCTL')])
 
 
+def bodies(sass):
+    body, cur = collections.OrderedDict(), None
+    for line in sass.splitlines():
+        m = re.search(r'Function : (\S+)', line)
+        if m:
+            cur = m.group(1)
+            body[cur] = []
+        elif cur:
+            m = re.search(r'/\*[0-9a-f]{4,}\*/\s*(.*?)\s*;', line)
+            if m:
+                body[cur].append(m.group(1))
+    # enum template arguments demangle as (lgr::Colour)0: keep the whole name
+    names = subprocess.run(['c++filt'], input='\n'.join(body), capture_output=True, text=True, check=True).stdout.split('\n')
+    for name, ins in zip(names, body.values()):
+        print(hashlib.sha256('\n'.join(ins).encode()).hexdigest()[:16], f'{len(ins):6d}', name)
+
+
 def main():
     sass = subprocess.run(['cuobjdump', '-sass', LIB], capture_output=True, text=True, check=True).stdout
+    if '--bodies' in sys.argv[1:]:
+        return bodies(sass)
     stats, cur = collections.OrderedDict(), None
     for line in sass.splitlines():
         m = re.search(r'Function : (\S+)', line)
