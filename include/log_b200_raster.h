@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 19
+#define LGR_ABI_VERSION 20
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -360,6 +360,33 @@ int lgr_point_compact(int64_t n, const int32_t* point_count_d, int32_t* scratch_
 int lgr_sparse_adam(int64_t rows, int32_t row_floats, const int64_t* index_d, const float* grad_d, float* param_d,
                     float* exp_avg_d, float* exp_avg_sq_d, float* max_exp_avg_sq_d, int64_t step, double lr, double beta1,
                     double beta2, double eps, void* stream);
+
+/* SSIM loss (LoG's training loss term, renderer.py:253-266): replaces LoG/render/loss.py:6-44 SSIM(11, C)(img1, img2)
+ * with reduce=True, i.e. 1 - mean(S) over the valid (B, C, H-10, W-10) map of
+ *     S = (2 mu1 mu2 + C1)(2 s12 + C2) / ((mu1^2 + mu2^2 + C1)(s11 + s22 + C2)),  C1 = 0.01^2, C2 = 0.03^2,
+ * mu / s the 11x11 Gaussian-window (sigma 1.5) means, variances and covariance of each plane, all in fp32.
+ *   img1_d, img2_d: fp32 images (B, C, H, W) read through the element strides strides1 / strides2 (HOST arrays of 4
+ *                   int64: B, C, H, W), so channels-last views and crops need no copy; batch, channels >= 1, H, W >= 11
+ *   scratch_d:      LGR_SSIM_SCRATCH_DOUBLES(B, C, H, W) doubles (per-CTA partial sums, summed in a fixed order: the loss
+ *                   repeats bit for bit)
+ *   loss_d:         (1) float, written on the device (no host synchronisation: capturable in a CUDA graph)
+ *   maps_d:         NULL, or LGR_SSIM_MAP_FLOATS(B, C, H, W) floats receiving dS/dmu1, dS/dE[x^2], dS/dE[xy] per map
+ *                   entry (three contiguous (B, C, H-10, W-10) blocks), which lgr_ssim_backward needs */
+#define LGR_SSIM_WINDOW 11
+#define LGR_SSIM_TILE 32
+#define LGR_SSIM_SCRATCH_DOUBLES(b, c, h, w) \
+  ((int64_t)(b) * (c) * (((h) - LGR_SSIM_WINDOW + LGR_SSIM_TILE) / LGR_SSIM_TILE) * (((w) - LGR_SSIM_WINDOW + LGR_SSIM_TILE) / LGR_SSIM_TILE))
+#define LGR_SSIM_MAP_FLOATS(b, c, h, w) (3 * (int64_t)(b) * (c) * ((h) - LGR_SSIM_WINDOW + 1) * ((w) - LGR_SSIM_WINDOW + 1))
+int lgr_ssim_forward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
+                     const int64_t* strides1, const float* img2_d, const int64_t* strides2, double* scratch_d, float* loss_d,
+                     float* maps_d, void* stream);
+/* Gradient of that loss w.r.t. img1: grad_img1_d (B, C, H, W) contiguous fp32 receives
+ *     dL/dx = g (w * P0 + 2 x (w * P1) + y (w * P2)),  g = -grad_loss_d[0] / (B C (H-10) (W-10)),
+ * with P0..P2 = maps_d of the forward and * the full 11x11 correlation (zero outside the map).  grad_loss_d: (1) float on
+ * the device (dL/dloss, never read on the host).  img1_d / img2_d / strides as in the forward. */
+int lgr_ssim_backward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
+                      const int64_t* strides1, const float* img2_d, const int64_t* strides2, const float* maps_d,
+                      const float* grad_loss_d, float* grad_img1_d, void* stream);
 
 /* Diagnostics (not on the data path): per-kernel CUDA-event timing on the launching stream.
  * lgr_profile_enable(1) starts recording; lgr_profile_collect() synchronises the recorded events, writes the summed

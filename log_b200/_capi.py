@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 19
+LGR_ABI_VERSION = 20
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -20,7 +20,8 @@ LGR_ROW_FLOATS = 20
 EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'lgr_forward_project',
            'lgr_forward_render', 'lgr_forward_render_device_sized', 'lgr_backward', 'lgr_grad_scatter_add', 'lgr_grad_scatter_add_staged', 'lgr_point_compact', 'lgr_sparse_adam', 'lgr_profile_enable', 'lgr_profile_collect',
            'lgr_profile_kernel_name', 'lgr_shard_send', 'lgr_shard_recv_bin', 'lgr_blend_backward', 'lgr_shard_return_rows',
-           'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible')
+           'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible',
+           'lgr_ssim_forward', 'lgr_ssim_backward')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -50,6 +51,20 @@ class LgrTree(ctypes.Structure):
 def tree_scratch_ints(num_points, slots):
     """LGR_TREE_SCRATCH_INTS."""
     return 8 + 2 * num_points + slots + 2 * ((slots + 255) // 256) + 2 + (slots + 3) // 4
+
+
+LGR_SSIM_WINDOW = 11
+LGR_SSIM_TILE = 32
+
+
+def ssim_scratch_doubles(b, c, h, w):
+    """LGR_SSIM_SCRATCH_DOUBLES."""
+    return b * c * ((h - LGR_SSIM_WINDOW + LGR_SSIM_TILE) // LGR_SSIM_TILE) * ((w - LGR_SSIM_WINDOW + LGR_SSIM_TILE) // LGR_SSIM_TILE)
+
+
+def ssim_map_floats(b, c, h, w):
+    """LGR_SSIM_MAP_FLOATS."""
+    return 3 * b * c * (h - LGR_SSIM_WINDOW + 1) * (w - LGR_SSIM_WINDOW + 1)
 
 
 def shard_send_ints(n_local, r):
@@ -109,6 +124,10 @@ def bind(lib):
     lib.lgr_tree_traverse.restype = ctypes.c_int
     lib.lgr_tree_traverse.argtypes = [ctypes.POINTER(LgrTree), _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _vp, _i64, _f32,
                                       _i32, _vp, _vp, _vp, _vp]
+    lib.lgr_ssim_forward.restype = ctypes.c_int
+    lib.lgr_ssim_forward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    lib.lgr_ssim_backward.restype = ctypes.c_int
+    lib.lgr_ssim_backward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     lib.lgr_profile_enable.restype = ctypes.c_int
     lib.lgr_profile_enable.argtypes = [ctypes.c_int]
     lib.lgr_profile_collect.restype = ctypes.c_int

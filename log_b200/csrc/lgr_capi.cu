@@ -35,6 +35,10 @@ int launch_shard_return(const ShardLayout&, const float*, int64_t, const void*, 
 int launch_shard_gather(const View&, const ShardLayout&, int64_t, const float*, const int32_t*, const int32_t*, const float*,
                         float*, float*, int32_t*, int, cudaStream_t);
 int launch_tree_traverse(const TreeArgs&, int64_t, int64_t, const int64_t*, int64_t, int, int32_t*, int64_t*, int64_t*, cudaStream_t);
+int launch_ssim_fwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, double*, float*, float*,
+                    cudaStream_t);
+int launch_ssim_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
+                    const float*, float*, cudaStream_t);
 }  // namespace lgr
 
 using namespace lgr;
@@ -237,6 +241,37 @@ int lgr_sparse_adam(int64_t rows, int32_t row_floats, const int64_t* index_d, co
   return launch_sparse_adam(rows, row_floats, index_d, grad_d, param_d, exp_avg_d, exp_avg_sq_d, max_exp_avg_sq_d,
                             (float)beta1, (float)beta2, (float)(1.0 - beta1), (float)(1.0 - beta2), (float)sqrt(bc2),
                             (float)(-step_size), (float)eps, (cudaStream_t)stream);
+}
+
+// Shape, pointers and strides of an lgr_ssim_* call; the grid (one CTA per 32x32 tile of every plane) must fit one dimension.
+static bool ssim_args_ok(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
+                         const int64_t* strides1, const float* img2_d, const int64_t* strides2) {
+  if (batch < 1 || channels < 1 || height < LGR_SSIM_WINDOW || width < LGR_SSIM_WINDOW) return false;
+  if (!img1_d || !img2_d || !strides1 || !strides2) return false;
+  for (int k = 0; k < 4; k++)
+    if (strides1[k] < 0 || strides2[k] < 0) return false;
+  const int64_t tiles = (int64_t)batch * channels * ((height + LGR_SSIM_TILE - 1) / LGR_SSIM_TILE) *
+                        ((width + LGR_SSIM_TILE - 1) / LGR_SSIM_TILE);
+  return tiles <= 0x7fffffff;
+}
+
+int lgr_ssim_forward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
+                     const int64_t* strides1, const float* img2_d, const int64_t* strides2, double* scratch_d, float* loss_d,
+                     float* maps_d, void* stream) {
+  if (!ssim_args_ok(batch, channels, height, width, img1_d, strides1, img2_d, strides2) || !scratch_d || !loss_d)
+    return LGR_E_BADARG;
+  return launch_ssim_fwd(batch, channels, height, width, img1_d, strides1, img2_d, strides2, scratch_d, loss_d, maps_d,
+                         (cudaStream_t)stream);
+}
+
+int lgr_ssim_backward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
+                      const int64_t* strides1, const float* img2_d, const int64_t* strides2, const float* maps_d,
+                      const float* grad_loss_d, float* grad_img1_d, void* stream) {
+  if (!ssim_args_ok(batch, channels, height, width, img1_d, strides1, img2_d, strides2) || !maps_d || !grad_loss_d ||
+      !grad_img1_d)
+    return LGR_E_BADARG;
+  return launch_ssim_bwd(batch, channels, height, width, img1_d, strides1, img2_d, strides2, maps_d, grad_loss_d,
+                         grad_img1_d, (cudaStream_t)stream);
 }
 
 int lgr_point_compact(int64_t n, const int32_t* point_count_d, int32_t* scratch_d, int32_t* ids_out_d,

@@ -249,6 +249,12 @@ def main():
     model.optimizer.step = fused_adam_step(model)
     res['base_stage_ms_per_iter_fused_adam'] = T.time(lambda: train_step(model, rend, batch), args.iters)
     model.optimizer.step = stock_step
+    # the same with LoG's SSIM loss on the fused kernels (INTEGRATION.md section 6: renderer.ssim_loss swapped)
+    from log_b200.loss import SSIM
+    stock_ssim = rend.ssim_loss
+    rend.ssim_loss = SSIM(11, 3).to(dev)
+    res['base_stage_ms_per_iter_fused_ssim'] = T.time(lambda: train_step(model, rend, batch), args.iters)
+    rend.ssim_loss = stock_ssim
 
     # ---- depth stage: LoG's Splitter creates child nodes; every iteration now walks the tree (prepare -> traverse) ----
     model.set_stage('depth')
