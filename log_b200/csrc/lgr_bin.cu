@@ -267,6 +267,9 @@ __device__ __forceinline__ void sort_tile(uint32_t* kA, uint32_t* vA, uint32_t* 
 //      to its final slot); larger bins are pushed on a block-level work stack and partitioned again.
 // Uniformly distributed depths finish after one partition (bins of ~L/256 entries).  No match.any / warp ranking:
 // the stable LSD sort kept below for huge lists spends its time in the ADU pipe on exactly those.
+#ifndef LGR_ON_LSD_FALLBACK
+#define LGR_ON_LSD_FALLBACK()     // test hook: the CPU emulation (tests/emu) counts the lists that reach the LSD sort
+#endif
 constexpr int MSD_SMALL = 96;     // rank counting is O(bin) per element with uniform SIMT control flow: cheap up to ~100
 constexpr int MSD_STACK = 512;
 
@@ -419,7 +422,10 @@ tile_sort_kernel(const int32_t* __restrict__ tile_list /* nullptr: tile = blockI
       uint32_t* kA = inst_key + beg; uint32_t* vA = inst_val + beg;
       uint32_t* kB = tmp + 2 * (int64_t)beg; uint32_t* vB = kB + len;
       __syncthreads();
-      if (!sort_tile_msd(kA, vA, kB, vB, len, msd)) sort_tile(kA, vA, kB, vB, len, id_bits, whist);
+      if (!sort_tile_msd(kA, vA, kB, vB, len, msd)) {
+        LGR_ON_LSD_FALLBACK();
+        sort_tile(kA, vA, kB, vB, len, id_bits, whist);
+      }
       for (int i = threadIdx.x; i < len; i += SORT_THREADS) sorted_ids[beg + i] = (int32_t)vA[i];
     }
     __syncthreads();      // the shared buffers are reused by the next tile of this CTA

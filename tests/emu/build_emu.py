@@ -119,7 +119,9 @@ def build(force=False, asan=None):
             fh.write(translate(open(os.path.join(CSRC, f)).read()))
         objs.append(cpp)
     # a 3-CTA grid for the tree walk: every emulated CTA costs 256 fibers, and 3 CTAs make the grid-stride loops iterate
-    cmd = ['g++', '-std=c++17', '-O1', '-g', '-fPIC', '-shared', '-w', '-DLGR_TREE_GRID=3', '-DLGR_REGION_GRID=2'] + extra + \
+    # and a counter of the tile lists that reach the LSD sort (tests/emu/cuda_runtime.h)
+    cmd = ['g++', '-std=c++17', '-O1', '-g', '-fPIC', '-shared', '-w', '-DLGR_TREE_GRID=3', '-DLGR_REGION_GRID=2',
+           '-DLGR_ON_LSD_FALLBACK()=emu_count_lsd_fallback()'] + extra + \
           (['-fsanitize=thread', '-DEMU_TSAN'] + (['-DEMU_TSAN_UNORDERED_CTAS'] if tsan == 2 else []) if tsan else ['-fsanitize=address', '-fno-omit-frame-pointer'] if asan else []) + ['-I', HERE, '-I', CSRC, '-o', LIB + '.tmp'] + objs + \
           [os.path.join(HERE, 'emu_api.cpp')]
     env = dict(os.environ)

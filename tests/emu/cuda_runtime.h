@@ -272,6 +272,11 @@ inline void __syncthreads() { emu::barrier_cta(); }
 inline void __syncwarp(unsigned = 0xffffffffu) { emu::barrier_warp(); }
 inline void __trap() { fprintf(stderr, "emu: __trap()\n"); abort(); }
 
+// LGR_ON_LSD_FALLBACK() in lgr_bin.cu (defined by build_emu.py): lists whose MSD work stack overflowed, so that a test can
+// prove it reached the LSD sort
+inline long long& emu_lsd_fallbacks() { static long long n = 0; return n; }
+inline void emu_count_lsd_fallback() { if (threadIdx.x == 0) emu_lsd_fallbacks()++; }
+
 EMU_NOTSAN inline int __syncthreads_reduce(int pred, int mode) {   // 0 or, 1 and, 2 count
   emu::Cta* c = emu::cta();
   // phase 1: everybody contributes

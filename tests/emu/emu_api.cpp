@@ -29,6 +29,8 @@ extern "C" {
 
 int emu_sort_smem_capacity(void) { return sort_smem_capacity(); }
 
+long long emu_lsd_fallback_count(void) { return emu_lsd_fallbacks(); }
+
 // tile_cursor holds the per-tile counts (stride CSTRIDE) on entry, as project_fwd leaves them
 int emu_tile_scan(const lgr_view* view, int32_t* tile_start, int32_t* tile_cursor, int32_t* meta) {
   const View v = make_view(view, 0);

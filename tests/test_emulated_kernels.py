@@ -136,7 +136,8 @@ def run_bin_and_sort(emu, view, rec, rad, counts):
     (112, 80, 3000, False, 40),       # 35 tiles, ordinary lists
     (112, 80, 4000, True, 60),        # depth ties / clusters: tie-break by id, MSD recursion on crowded digits
     (16, 16, 5000, True, 30),         # one tile, list > 4096: the long-tile launch (large shared-memory sort)
-    (16, 16, 16500, False, 30),       # one tile, list > 13312: the stable LSD fallback over global scratch
+    (16, 16, 16500, False, 30),       # one tile, list > 13312: the MSD sort over global scratch (its LSD fallback:
+                                      # tests/test_scale_paths.py)
     (40, 33, 0, False, 10),           # empty input
 ])
 def test_scan_scatter_sort_emulated(emu, W, H, n, clustered, max_rad):
@@ -182,6 +183,12 @@ def shard_world(n, H, W, world):
 
 @pytest.mark.parametrize('world,W,H,n', [(3, 112, 80, 1500), (2, 64, 48, 700), (4, 96, 40, 300), (8, 64, 144, 2100)])
 def test_shard_exchange_emulated(emu, world, W, H, n):
+    run_shard_exchange(emu, world, W, H, n)
+
+
+def run_shard_exchange(emu, world, W, H, n, max_rads=(45, 12)):
+    """Two steps through the same exchange buffers (the largest splat radius of each step: max_rads): push, receive + bin +
+    sort, return, gather, each compared with a numpy restatement."""
     from log_b200 import _capi
     gx, gy = (W + 15) // 16, (H + 15) // 16
     lays, bufs, peers, parts, bands = shard_world(n, H, W, world)
@@ -190,7 +197,7 @@ def test_shard_exchange_emulated(emu, world, W, H, n):
     full = make_view(H, W)
     rng = np.random.default_rng(99)
     dsplat = [np.full((rows, 12), 7.0, dtype=F) for _ in range(world)]              # garbage: used rows must be zeroed
-    for step, (seed, max_rad) in enumerate(((1, 45), (2, 12))):                      # step 2: fewer rows -> stale slots
+    for step, (seed, max_rad) in enumerate(zip((1, 2), max_rads)):                  # step 2: fewer rows -> stale slots
         rec, rad = make_records(n, W, H, seed=seed, clustered=(step == 1), max_rad=max_rad)
         x0, y0, x1, y1, _ = tile_rects(rec[:, 0], rec[:, 1], rad, rec[:, 6], rec[:, 7], gx, gy, 0, gy)
         use = (rad > 0) & (rec[:, 6] > 0) & (x1 > x0) & (y1 > y0)

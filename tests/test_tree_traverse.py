@@ -7,7 +7,8 @@ several (min_resolution_pixel, max_depth, root subset) queries (generator: tests
   * CPU: the real kernel source on the SIMT emulation (tests/emu) reproduces every golden list exactly, and agrees with
     the oracle on scenes with culled points (where the reference's PyTorch twin and its CUDA kernel differ: the kernel,
     which LoG actually runs, returns radius 0 for points outside +-1.3 NDC);
-  * `-m gpu`: the same on hardware (tests/test_zz_gpu_tree.py)."""
+  * `-m gpu`: the same on hardware (tests/test_zz_gpu_new_rows.py).
+Forests large enough to reach the walk's scan carry and grid strides: tests/test_scale_paths.py."""
 import math
 import os
 import types
@@ -74,6 +75,17 @@ def make_objects(ti, dev, min_px):
     return tree, model, types.SimpleNamespace(raster_settings=settings)
 
 
+def stand_ins(cam, dev, node_index, table, C, max_level, min_px, xyz, scal, rot):
+    """The same stand-ins for a synthetic forest (numpy arrays; parameters rounded to float32) seen by camera `cam`."""
+    from util import settings_from_camera
+    tree = types.SimpleNamespace(node_index=torch.from_numpy(node_index).to(dev), tree=torch.from_numpy(table).to(dev), max_child=C,
+                                 max_level=max_level, min_resolution_pixel=min_px)
+    t32 = lambda a: torch.from_numpy(a).to(device=dev, dtype=torch.float32)
+    model = types.SimpleNamespace(xyz=t32(xyz), scaling=t32(scal), rotation=t32(rot),
+                                  activation=types.SimpleNamespace(scaling_activation=torch.exp))
+    return tree, model, types.SimpleNamespace(raster_settings=settings_from_camera(cam, dev))
+
+
 def check_goldens():
     from log_b200.tree import traverse
     dev = device()
@@ -121,12 +133,7 @@ def check_culled_scene_against_oracle(seed=5):
     xyz, scal, rot = f(xyz), f(scal), f(rot)
     node_index, table = np.array(node_index, np.int32), np.array(table, np.int32).reshape(-1, C)
     roots = np.nonzero(rng.random(n_root) < 0.8)[0].astype(np.int64)
-    tree = types.SimpleNamespace(node_index=torch.from_numpy(node_index).to(dev), tree=torch.from_numpy(table).to(dev), max_child=C,
-                                 max_level=20, min_resolution_pixel=3.0)
-    t32 = lambda a: torch.from_numpy(a).to(device=dev, dtype=torch.float32)
-    model = types.SimpleNamespace(xyz=t32(xyz), scaling=t32(scal), rotation=t32(rot),
-                                  activation=types.SimpleNamespace(scaling_activation=torch.exp))
-    _, _, rast = make_objects(0, dev, 3.0)
+    tree, model, rast = stand_ins(cam, dev, node_index, table, C, 20, 3.0, xyz, scal, rot)
     for max_depth in (1000, 3, 1):
         want, radii = tree_oracle.traverse(cam, node_index, table, 20, 3.0, xyz, scal, rot, roots, max_depth=max_depth, return_radii=True)
         assert (radii == 0).sum() > 20 and (np.abs(radii[radii > 0] / 3.0 - 1.0) > 1e-4).all()
