@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 20
+#define LGR_ABI_VERSION 21
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -387,6 +387,47 @@ int lgr_ssim_forward(int32_t batch, int32_t channels, int32_t height, int32_t wi
 int lgr_ssim_backward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
                       const int64_t* strides1, const float* img2_d, const int64_t* strides2, const float* maps_d,
                       const float* grad_loss_d, float* grad_img1_d, void* stream);
+
+/* Depth-supervision loss (LoG's NaiveRendererAndLoss.append_depth_loss, renderer.py:268-292, with MiDaS's
+ * ScaleAndShiftInvariantLoss(alpha=0.5, scales=1), LoG/render/loss.py:47-117).  For each of the 64 patches k, the 64x64
+ * window at (start_rows_d[k], start_cols_d[k]) of the three maps, with m = accmap > 0.5, q = 1/(pred + 1e-5), g = gt:
+ *     (s, t) the least-squares fit of s q + t to g over the masked pixels (s = t = 0 where its determinant is 0),
+ *     r = s q + t - g,   loss = [sum m r^2 + 0.5 sum_{neighbour pairs in a patch} m_i m_j |r_j - r_i|] / M,
+ * M the masked pixels over all patches (overlaps count twice); moments and fit in fp64 about a local centre.
+ *   pred_d, accmap_d:  fp32 (height, width) maps read through the element strides pred_strides / acc_strides (HOST
+ *                      arrays of 2 int64: row, column), so planes of a (6, H, W) render need no copy
+ *   gt_d:              fp32 (gt_height, gt_width) ground truth, strides gt_strides; 64 <= gt_height <= height,
+ *                      64 <= gt_width <= width (the patches index every map at the ground truth's coordinates)
+ *   start_rows_d / start_cols_d: LGR_DEPTH_PATCHES int64 corners on the device.  A corner whose patch does not lie inside
+ *                      the ground truth reads nothing and makes the loss (and the gradient it covers) NaN.
+ *   stats_d:           LGR_DEPTH_STAT_DOUBLES doubles: per-patch fit and partial sums, which lgr_depth_loss_backward needs
+ *   loss_d:            (1) float, written on the device (no host synchronisation: capturable in a CUDA graph).  An empty
+ *                      mask gives NaN (0/0).  Sums are in a fixed order: the loss repeats bit for bit. */
+#define LGR_DEPTH_PATCHES 64
+#define LGR_DEPTH_PATCH 64
+#define LGR_DEPTH_STAT_DOUBLES_PER_PATCH 8
+#define LGR_DEPTH_STAT_DOUBLES (LGR_DEPTH_STAT_DOUBLES_PER_PATCH * LGR_DEPTH_PATCHES + 8)
+#define LGR_DEPTH_GRAD_SCRATCH_FLOATS ((int64_t)LGR_DEPTH_PATCHES * LGR_DEPTH_PATCH * LGR_DEPTH_PATCH)
+#define LGR_DEPTH_VIS_GRID 264
+#define LGR_DEPTH_VIS_SCRATCH_FLOATS (2 * LGR_DEPTH_VIS_GRID)
+int lgr_depth_loss_forward(int32_t height, int32_t width, int32_t gt_height, int32_t gt_width, const float* pred_d,
+                           const int64_t* pred_strides, const float* accmap_d, const int64_t* acc_strides, const float* gt_d,
+                           const int64_t* gt_strides, const int64_t* start_rows_d, const int64_t* start_cols_d,
+                           double* stats_d, float* loss_d, void* stream);
+/* Gradient of that loss w.r.t. pred: grad_pred_d (height, width) contiguous fp32 receives, per pixel, grad_loss_d[0] / M
+ * times the sum of dL_k/dpred over the patches covering it (in patch order, no atomics), 0 where none does.  It includes
+ * the paths through s and t.  grad_scratch_d: LGR_DEPTH_GRAD_SCRATCH_FLOATS floats; stats_d from the forward;
+ * grad_loss_d (1) float on the device.  The other arguments as in the forward. */
+int lgr_depth_loss_backward(int32_t height, int32_t width, int32_t gt_height, int32_t gt_width, const float* pred_d,
+                            const int64_t* pred_strides, const float* accmap_d, const int64_t* acc_strides,
+                            const float* gt_d, const int64_t* gt_strides, const int64_t* start_rows_d,
+                            const int64_t* start_cols_d, const double* stats_d, float* grad_scratch_d,
+                            const float* grad_loss_d, float* grad_pred_d, void* stream);
+/* LoG's depth visualisation: vis_d (height, width) contiguous fp32 receives (q - min q) / (max q - min q), q = 1/(pred +
+ * 1e-5) in fp32, min and max over the pixels with accmap > 0.5 -- bit for bit torch's fp32 result.  An empty mask gives
+ * NaN everywhere (LoG raises there).  scratch_d: LGR_DEPTH_VIS_SCRATCH_FLOATS floats. */
+int lgr_depth_vis(int32_t height, int32_t width, const float* pred_d, const int64_t* pred_strides, const float* accmap_d,
+                  const int64_t* acc_strides, float* scratch_d, float* vis_d, void* stream);
 
 /* Diagnostics (not on the data path): per-kernel CUDA-event timing on the launching stream.
  * lgr_profile_enable(1) starts recording; lgr_profile_collect() synchronises the recorded events, writes the summed

@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 20
+LGR_ABI_VERSION = 21
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -21,7 +21,7 @@ EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'l
            'lgr_forward_render', 'lgr_forward_render_device_sized', 'lgr_backward', 'lgr_grad_scatter_add', 'lgr_grad_scatter_add_staged', 'lgr_point_compact', 'lgr_sparse_adam', 'lgr_profile_enable', 'lgr_profile_collect',
            'lgr_profile_kernel_name', 'lgr_shard_send', 'lgr_shard_recv_bin', 'lgr_blend_backward', 'lgr_shard_return_rows',
            'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible',
-           'lgr_ssim_forward', 'lgr_ssim_backward')
+           'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -65,6 +65,15 @@ def ssim_scratch_doubles(b, c, h, w):
 def ssim_map_floats(b, c, h, w):
     """LGR_SSIM_MAP_FLOATS."""
     return 3 * b * c * (h - LGR_SSIM_WINDOW + 1) * (w - LGR_SSIM_WINDOW + 1)
+
+
+LGR_DEPTH_PATCHES = 64
+LGR_DEPTH_PATCH = 64
+LGR_DEPTH_STAT_DOUBLES_PER_PATCH = 8
+LGR_DEPTH_STAT_DOUBLES = LGR_DEPTH_STAT_DOUBLES_PER_PATCH * LGR_DEPTH_PATCHES + 8
+LGR_DEPTH_GRAD_SCRATCH_FLOATS = LGR_DEPTH_PATCHES * LGR_DEPTH_PATCH * LGR_DEPTH_PATCH
+LGR_DEPTH_VIS_GRID = 264
+LGR_DEPTH_VIS_SCRATCH_FLOATS = 2 * LGR_DEPTH_VIS_GRID
 
 
 def shard_send_ints(n_local, r):
@@ -128,6 +137,12 @@ def bind(lib):
     lib.lgr_ssim_forward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     lib.lgr_ssim_backward.restype = ctypes.c_int
     lib.lgr_ssim_backward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    lib.lgr_depth_loss_forward.restype = ctypes.c_int
+    lib.lgr_depth_loss_forward.argtypes = [_i32, _i32, _i32, _i32] + [_vp] * 11
+    lib.lgr_depth_loss_backward.restype = ctypes.c_int
+    lib.lgr_depth_loss_backward.argtypes = [_i32, _i32, _i32, _i32] + [_vp] * 13
+    lib.lgr_depth_vis.restype = ctypes.c_int
+    lib.lgr_depth_vis.argtypes = [_i32, _i32] + [_vp] * 7
     lib.lgr_profile_enable.restype = ctypes.c_int
     lib.lgr_profile_enable.argtypes = [ctypes.c_int]
     lib.lgr_profile_collect.restype = ctypes.c_int

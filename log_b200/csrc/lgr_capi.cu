@@ -39,6 +39,12 @@ int launch_ssim_fwd(int, int, int, int, const float*, const int64_t*, const floa
                     cudaStream_t);
 int launch_ssim_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
                     const float*, float*, cudaStream_t);
+int launch_depth_loss_fwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
+                          const int64_t*, const int64_t*, const int64_t*, double*, float*, cudaStream_t);
+int launch_depth_loss_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
+                          const int64_t*, const int64_t*, const int64_t*, const double*, float*, const float*, float*,
+                          cudaStream_t);
+int launch_depth_vis(int, int, const float*, const int64_t*, const float*, const int64_t*, float*, float*, cudaStream_t);
 }  // namespace lgr
 
 using namespace lgr;
@@ -272,6 +278,52 @@ int lgr_ssim_backward(int32_t batch, int32_t channels, int32_t height, int32_t w
     return LGR_E_BADARG;
   return launch_ssim_bwd(batch, channels, height, width, img1_d, strides1, img2_d, strides2, maps_d, grad_loss_d,
                          grad_img1_d, (cudaStream_t)stream);
+}
+
+// Shapes, pointers and strides of an lgr_depth_loss_* call: the patches index all three maps at the ground truth's
+// coordinates, so the prediction must be at least as large; the dense gradient's grid strides over height * width.
+static bool depth_args_ok(int32_t height, int32_t width, int32_t gt_height, int32_t gt_width, const float* pred_d,
+                          const int64_t* pred_strides, const float* accmap_d, const int64_t* acc_strides, const float* gt_d,
+                          const int64_t* gt_strides, const int64_t* start_rows_d, const int64_t* start_cols_d) {
+  if (gt_height < LGR_DEPTH_PATCH || gt_width < LGR_DEPTH_PATCH || height < gt_height || width < gt_width) return false;
+  if (!pred_d || !accmap_d || !gt_d || !pred_strides || !acc_strides || !gt_strides || !start_rows_d || !start_cols_d)
+    return false;
+  for (int k = 0; k < 2; k++)
+    if (pred_strides[k] < 0 || acc_strides[k] < 0 || gt_strides[k] < 0) return false;
+  return true;
+}
+
+int lgr_depth_loss_forward(int32_t height, int32_t width, int32_t gt_height, int32_t gt_width, const float* pred_d,
+                           const int64_t* pred_strides, const float* accmap_d, const int64_t* acc_strides, const float* gt_d,
+                           const int64_t* gt_strides, const int64_t* start_rows_d, const int64_t* start_cols_d,
+                           double* stats_d, float* loss_d, void* stream) {
+  if (!depth_args_ok(height, width, gt_height, gt_width, pred_d, pred_strides, accmap_d, acc_strides, gt_d, gt_strides,
+                     start_rows_d, start_cols_d) || !stats_d || !loss_d)
+    return LGR_E_BADARG;
+  return launch_depth_loss_fwd(height, width, gt_height, gt_width, pred_d, pred_strides, accmap_d, acc_strides, gt_d,
+                               gt_strides, start_rows_d, start_cols_d, stats_d, loss_d, (cudaStream_t)stream);
+}
+
+int lgr_depth_loss_backward(int32_t height, int32_t width, int32_t gt_height, int32_t gt_width, const float* pred_d,
+                            const int64_t* pred_strides, const float* accmap_d, const int64_t* acc_strides,
+                            const float* gt_d, const int64_t* gt_strides, const int64_t* start_rows_d,
+                            const int64_t* start_cols_d, const double* stats_d, float* grad_scratch_d,
+                            const float* grad_loss_d, float* grad_pred_d, void* stream) {
+  if (!depth_args_ok(height, width, gt_height, gt_width, pred_d, pred_strides, accmap_d, acc_strides, gt_d, gt_strides,
+                     start_rows_d, start_cols_d) || !stats_d || !grad_scratch_d || !grad_loss_d || !grad_pred_d)
+    return LGR_E_BADARG;
+  return launch_depth_loss_bwd(height, width, gt_height, gt_width, pred_d, pred_strides, accmap_d, acc_strides, gt_d,
+                               gt_strides, start_rows_d, start_cols_d, stats_d, grad_scratch_d, grad_loss_d, grad_pred_d,
+                               (cudaStream_t)stream);
+}
+
+int lgr_depth_vis(int32_t height, int32_t width, const float* pred_d, const int64_t* pred_strides, const float* accmap_d,
+                  const int64_t* acc_strides, float* scratch_d, float* vis_d, void* stream) {
+  if (height < 1 || width < 1 || !pred_d || !pred_strides || !accmap_d || !acc_strides || !scratch_d || !vis_d)
+    return LGR_E_BADARG;
+  for (int k = 0; k < 2; k++)
+    if (pred_strides[k] < 0 || acc_strides[k] < 0) return LGR_E_BADARG;
+  return launch_depth_vis(height, width, pred_d, pred_strides, accmap_d, acc_strides, scratch_d, vis_d, (cudaStream_t)stream);
 }
 
 int lgr_point_compact(int64_t n, const int32_t* point_count_d, int32_t* scratch_d, int32_t* ids_out_d,
