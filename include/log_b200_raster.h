@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 21
+#define LGR_ABI_VERSION 22
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -360,6 +360,63 @@ int lgr_point_compact(int64_t n, const int32_t* point_count_d, int32_t* scratch_
 int lgr_sparse_adam(int64_t rows, int32_t row_floats, const int64_t* index_d, const float* grad_d, float* param_d,
                     float* exp_avg_d, float* exp_avg_sq_d, float* max_exp_avg_sq_d, int64_t step, double lr, double beta1,
                     double beta2, double eps, void* stream);
+
+/* LoG's per-Gaussian training statistics (Counter, LoG/model/counter.py:4-19): eight (N) tables on the device. */
+typedef struct lgr_counter {
+  int32_t* create_steps_d;
+  int16_t* visible_count_d;
+  float* weights_max_d;
+  float* weights_sum_d;
+  int16_t* radii_max_d;
+  int32_t* area_sum_d;
+  float* grad_sum_d;
+  int32_t* radii_max_max_d;
+} lgr_counter;
+/* One view of Counter.update_by_output (counter.py:36-68).  Rendered row r < num_leaf + num_node is Gaussian
+ * g(r) = r < num_leaf ? index_leaf_d[r] : index_node_d[r - num_leaf] (int64).  For every row:
+ *     flag_vis_d[r] = radii_d[r] > 0  (uint8 0/1, the bytes of a torch.bool tensor), and where it is set
+ *     create_steps += 1, visible_count += 1 (int16, wraps), weights_max = max(weights_max, point_weight_d[r]) (NaN
+ *     propagates, as torch.max), weights_sum += point_weight_d[r], radii_max = max(radii_max, (int16)radii_d[r]);
+ * for every j < num_points, with p = point_id_d[j], c = point_count_d[j] and g = g(p):
+ *     area_sum += c (mod 2^32), grad_sum += |(grad[p][0], grad[p][1])|_2 * (float)c, radii_max_max = max((int32)c, .).
+ *   radii_d int32, point_weight_d float32 (rows); grad_d float32 (rows, >= 2) read at grad_strides (HOST, 2 int64 elements).
+ *   point_id_d / point_count_d: int32 or int64 (id_bytes / count_bytes = 4 or 8).
+ * Plain read-modify-writes, no atomics: the g(r) must be unique and the point ids unique, or all equal with count 0 (the
+ * stock rasteriser's zero vectors, where every thread writes the same value).  Equal inputs give bit-identical counters. */
+int lgr_counter_update(const lgr_counter* counter, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
+                       const int64_t* index_node_d, const int32_t* radii_d, const float* point_weight_d, const float* grad_d,
+                       const int64_t* grad_strides, int64_t num_points, const void* point_id_d, const void* point_count_d,
+                       int32_t id_bytes, int32_t count_bytes, uint8_t* flag_vis_d, void* stream);
+
+/* One key of LoG.step (level_of_gaussian.py:379-398): the parameter table getattr(gaussian, key) and its optimiser state,
+ * all (N, row_floats) float32 contiguous, and the compact (rows, row_floats) gradient of the gathered rows. */
+#define LGR_STEP_MAX_KEYS 8
+typedef struct lgr_step_key {
+  float* param_d;
+  float* exp_avg_d;
+  float* exp_avg_sq_d;
+  float* max_exp_avg_sq_d; /* NULL: no amsgrad */
+  const float* grad_d;     /* NULL: the key has no gradient, Adam leaves it alone */
+  int32_t row_floats;
+  int32_t prefix;          /* floats of the keys before it: the key owns columns [prefix, prefix + row_floats) of a row */
+  float neg_step_size;     /* -lr / (1 - beta1^step), computed by the caller */
+  float bc2_sqrt;          /* sqrt(1 - beta2^step) */
+  int32_t clamp;           /* 1 for scaling (row_floats 3): clamp to [log radius3d_min, log radius3d_max] after Adam */
+} lgr_step_key;
+typedef struct lgr_step {
+  lgr_step_key keys[LGR_STEP_MAX_KEYS];
+  int32_t num_keys;
+  int32_t row_floats;      /* sum of the keys' row_floats */
+  float beta1, beta2, one_minus_beta1, one_minus_beta2, eps;
+  const float* radius3d_min_d; /* (N) Counter.radius3d_min / radius3d_max, read by the clamp */
+  const float* radius3d_max_d;
+} lgr_step;
+/* SparseOptimizer.step + LoG.clamp_scale for rows r < num_leaf + num_node with flag_vis_d[r] (uint8), on Gaussian g(r)
+ * as in lgr_counter_update: per key with a gradient the update of lgr_sparse_adam on row g(r) with grad_d[r], then for
+ * the clamp key min(max(s, logf(radius3d_min[g])), logf(radius3d_max[g])) (NaN propagates, as torch.clamp).  Rows
+ * without flag_vis are not touched.  The g(r) of flagged rows must be unique.  One launch for every key. */
+int lgr_log_step(const lgr_step* step, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
+                 const int64_t* index_node_d, const uint8_t* flag_vis_d, void* stream);
 
 /* SSIM loss (LoG's training loss term, renderer.py:253-266): replaces LoG/render/loss.py:6-44 SSIM(11, C)(img1, img2)
  * with reduce=True, i.e. 1 - mean(S) over the valid (B, C, H-10, W-10) map of

@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 21
+LGR_ABI_VERSION = 22
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -21,7 +21,8 @@ EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'l
            'lgr_forward_render', 'lgr_forward_render_device_sized', 'lgr_backward', 'lgr_grad_scatter_add', 'lgr_grad_scatter_add_staged', 'lgr_point_compact', 'lgr_sparse_adam', 'lgr_profile_enable', 'lgr_profile_collect',
            'lgr_profile_kernel_name', 'lgr_shard_send', 'lgr_shard_recv_bin', 'lgr_blend_backward', 'lgr_shard_return_rows',
            'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible',
-           'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis')
+           'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis',
+           'lgr_counter_update', 'lgr_log_step')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -79,6 +80,28 @@ LGR_DEPTH_VIS_SCRATCH_FLOATS = 2 * LGR_DEPTH_VIS_GRID
 def shard_send_ints(n_local, r):
     """LGR_SHARD_SEND_INTS: int32 scratch of lgr_shard_send (kept until lgr_shard_gather)."""
     return 2 * r * ((max(n_local, 1) + 255) // 256) + r
+
+
+class LgrCounter(ctypes.Structure):
+    """struct lgr_counter: LoG's eight Counter tables."""
+    _fields_ = [('create_steps_d', _vp), ('visible_count_d', _vp), ('weights_max_d', _vp), ('weights_sum_d', _vp),
+                ('radii_max_d', _vp), ('area_sum_d', _vp), ('grad_sum_d', _vp), ('radii_max_max_d', _vp)]
+
+
+LGR_STEP_MAX_KEYS = 8
+
+
+class LgrStepKey(ctypes.Structure):
+    """struct lgr_step_key: one parameter table of LoG.step."""
+    _fields_ = [('param_d', _vp), ('exp_avg_d', _vp), ('exp_avg_sq_d', _vp), ('max_exp_avg_sq_d', _vp), ('grad_d', _vp),
+                ('row_floats', _i32), ('prefix', _i32), ('neg_step_size', _f32), ('bc2_sqrt', _f32), ('clamp', _i32)]
+
+
+class LgrStep(ctypes.Structure):
+    """struct lgr_step: the key table of lgr_log_step."""
+    _fields_ = [('keys', LgrStepKey * LGR_STEP_MAX_KEYS), ('num_keys', _i32), ('row_floats', _i32), ('beta1', _f32),
+                ('beta2', _f32), ('one_minus_beta1', _f32), ('one_minus_beta2', _f32), ('eps', _f32),
+                ('radius3d_min_d', _vp), ('radius3d_max_d', _vp)]
 
 
 class LgrError(RuntimeError):
@@ -143,6 +166,11 @@ def bind(lib):
     lib.lgr_depth_loss_backward.argtypes = [_i32, _i32, _i32, _i32] + [_vp] * 13
     lib.lgr_depth_vis.restype = ctypes.c_int
     lib.lgr_depth_vis.argtypes = [_i32, _i32] + [_vp] * 7
+    lib.lgr_counter_update.restype = ctypes.c_int
+    lib.lgr_counter_update.argtypes = [ctypes.POINTER(LgrCounter), _i64, _i64] + [_vp] * 6 + [_i64, _vp, _vp, _i32, _i32,
+                                                                                              _vp, _vp]
+    lib.lgr_log_step.restype = ctypes.c_int
+    lib.lgr_log_step.argtypes = [ctypes.POINTER(LgrStep), _i64, _i64, _vp, _vp, _vp, _vp]
     lib.lgr_profile_enable.restype = ctypes.c_int
     lib.lgr_profile_enable.argtypes = [ctypes.c_int]
     lib.lgr_profile_collect.restype = ctypes.c_int

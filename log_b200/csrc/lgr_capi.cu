@@ -24,6 +24,9 @@ int launch_blend_fwd(const View&, const int32_t*, const int32_t*, const float*, 
                      float*, float*, int32_t*, cudaStream_t);
 int launch_sparse_adam(int64_t, int, const int64_t*, const float*, float*, float*, float*, float*, float, float, float, float,
                        float, float, float, cudaStream_t);
+int launch_counter_update(const lgr_counter&, int64_t, int64_t, const int64_t*, const int64_t*, const int32_t*, const float*,
+                          const float*, const int64_t*, int64_t, const void*, const void*, int, int, uint8_t*, cudaStream_t);
+int launch_log_step(const lgr_step&, int64_t, int64_t, const int64_t*, const int64_t*, const uint8_t*, cudaStream_t);
 int launch_point_compact(int64_t, const int32_t*, int32_t*, int32_t*, int32_t*, int32_t*, cudaStream_t);
 int launch_blend_bwd(const View&, const int32_t*, const int32_t*, const float*, const float*, const float*, float*,
                      cudaStream_t);
@@ -247,6 +250,42 @@ int lgr_sparse_adam(int64_t rows, int32_t row_floats, const int64_t* index_d, co
   return launch_sparse_adam(rows, row_floats, index_d, grad_d, param_d, exp_avg_d, exp_avg_sq_d, max_exp_avg_sq_d,
                             (float)beta1, (float)beta2, (float)(1.0 - beta1), (float)(1.0 - beta2), (float)sqrt(bc2),
                             (float)(-step_size), (float)eps, (cudaStream_t)stream);
+}
+
+int lgr_counter_update(const lgr_counter* counter, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
+                       const int64_t* index_node_d, const int32_t* radii_d, const float* point_weight_d, const float* grad_d,
+                       const int64_t* grad_strides, int64_t num_points, const void* point_id_d, const void* point_count_d,
+                       int32_t id_bytes, int32_t count_bytes, uint8_t* flag_vis_d, void* stream) {
+  if (!counter || num_leaf < 0 || num_node < 0 || num_points < 0 || !grad_strides) return LGR_E_BADARG;
+  if ((id_bytes != 4 && id_bytes != 8) || (count_bytes != 4 && count_bytes != 8)) return LGR_E_BADARG;
+  if ((num_leaf > 0 && !index_leaf_d) || (num_node > 0 && !index_node_d)) return LGR_E_BADARG;
+  const lgr_counter& c = *counter;
+  if (!c.create_steps_d || !c.visible_count_d || !c.weights_max_d || !c.weights_sum_d || !c.radii_max_d || !c.area_sum_d ||
+      !c.grad_sum_d || !c.radii_max_max_d)
+    return LGR_E_BADARG;
+  if (num_leaf + num_node > 0 && (!radii_d || !point_weight_d || !flag_vis_d)) return LGR_E_BADARG;
+  if (num_points > 0 && (!point_id_d || !point_count_d || !grad_d || grad_strides[0] < 0 || grad_strides[1] < 0))
+    return LGR_E_BADARG;
+  return launch_counter_update(c, num_leaf, num_node, index_leaf_d, index_node_d, radii_d, point_weight_d, grad_d,
+                               grad_strides, num_points, point_id_d, point_count_d, id_bytes, count_bytes, flag_vis_d,
+                               (cudaStream_t)stream);
+}
+
+int lgr_log_step(const lgr_step* step, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
+                 const int64_t* index_node_d, const uint8_t* flag_vis_d, void* stream) {
+  if (!step || num_leaf < 0 || num_node < 0 || step->num_keys < 1 || step->num_keys > LGR_STEP_MAX_KEYS) return LGR_E_BADARG;
+  if ((num_leaf > 0 && !index_leaf_d) || (num_node > 0 && !index_node_d) || (num_leaf + num_node > 0 && !flag_vis_d))
+    return LGR_E_BADARG;
+  int32_t prefix = 0;
+  for (int k = 0; k < step->num_keys; k++) {      // the keys tile a row in order
+    const lgr_step_key& key = step->keys[k];
+    if (key.row_floats <= 0 || key.prefix != prefix || !key.param_d) return LGR_E_BADARG;
+    if (key.grad_d && (!key.exp_avg_d || !key.exp_avg_sq_d)) return LGR_E_BADARG;
+    if (key.clamp && (key.row_floats != 3 || !step->radius3d_min_d || !step->radius3d_max_d)) return LGR_E_BADARG;
+    prefix += key.row_floats;
+  }
+  if (prefix != step->row_floats) return LGR_E_BADARG;
+  return launch_log_step(*step, num_leaf, num_node, index_leaf_d, index_node_d, flag_vis_d, (cudaStream_t)stream);
 }
 
 // Shape, pointers and strides of an lgr_ssim_* call; the grid (one CTA per 32x32 tile of every plane) must fit one dimension.

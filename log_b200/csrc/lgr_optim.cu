@@ -1,8 +1,14 @@
-// Fused sparse Adam step for the Gaussians that were visible in the step (SURVEY.md 8(f) row 4).
+// Fused sparse Adam step for the Gaussians that were visible in the step (SURVEY.md 8(f) row 4), and LoG's whole
+// post-backward bookkeeping built on it.
 // Reference: LoG/model/sparse_optimizer.py:41-78 (_single_tensor_adam) applied to gathered rows and scattered back
 // (:163-196).  One pass: gather moments by index, update, write parameter and moments back in place.  28 bytes of HBM
 // traffic per element (32 with amsgrad); the reference runs ~10 elementwise torch kernels per parameter on gathered
 // copies plus an index.cpu() synchronisation.
+//   sparse_adam_kernel     one key, one thread per (row, float)
+//   counter_update_kernel  Counter.update_by_output (LoG/model/counter.py:36-68) for one view: one thread per rendered
+//                          row, then one per point_id entry; plain read-modify-writes on unique rows
+//   log_step_kernel        LoG.step (level_of_gaussian.py:379-398): every key's Adam update and the scale clamp
+//                          (:367-377), one thread per (row, float) across all keys
 #include "lgr_common.cuh"
 #include "lgr_prof.cuh"
 
@@ -10,26 +16,39 @@ namespace lgr {
 
 constexpr int ADAM_THREADS = 256;
 
+#ifndef __grid_constant__
+#define __grid_constant__      // host compilers of the kernel source: a kernel argument is an ordinary value there
+#endif
+
+struct AdamConst {
+  float beta1, beta2, one_minus_beta1, one_minus_beta2, bc2_sqrt, neg_step_size, eps;
+};
+
+// The update of one element, shared by sparse_adam_kernel and log_step_kernel.
+__device__ __forceinline__ void adam_element(float g, float* __restrict__ param, float* __restrict__ exp_avg,
+                                             float* __restrict__ exp_avg_sq, float* __restrict__ max_exp_avg_sq,
+                                             const AdamConst& a) {
+  // explicitly rounded, in the reference's order: m = m*b1 + (1-b1)*g ; v = v*b2 + ((1-b2)*g)*g
+  const float m = __fadd_rn(__fmul_rn(*exp_avg, a.beta1), __fmul_rn(a.one_minus_beta1, g));
+  const float v = __fadd_rn(__fmul_rn(*exp_avg_sq, a.beta2), __fmul_rn(__fmul_rn(a.one_minus_beta2, g), g));
+  *exp_avg = m;
+  *exp_avg_sq = v;
+  float vv = v;
+  if (max_exp_avg_sq) { vv = fmaxf(*max_exp_avg_sq, v); *max_exp_avg_sq = vv; }
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vv), a.bc2_sqrt), a.eps);
+  *param = __fadd_rn(*param, __fmul_rn(a.neg_step_size, __fdiv_rn(m, denom)));
+}
+
 __global__ void __launch_bounds__(ADAM_THREADS)
 sparse_adam_kernel(int64_t total, int C, const int64_t* __restrict__ index, const float* __restrict__ grad,
                    float* __restrict__ param, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
-                   float* __restrict__ max_exp_avg_sq, float beta1, float beta2, float one_minus_beta1,
-                   float one_minus_beta2, float bias_correction2_sqrt, float neg_step_size, float eps) {
+                   float* __restrict__ max_exp_avg_sq, AdamConst a) {
   const int64_t t = (int64_t)blockIdx.x * ADAM_THREADS + threadIdx.x;
   if (t >= total) return;
   const int64_t row = t / C;
   const int col = (int)(t - row * C);
   const int64_t dst = index[row] * C + col;
-  const float g = __ldg(grad + t);
-  // explicitly rounded, in the reference's order: m = m*b1 + (1-b1)*g ; v = v*b2 + ((1-b2)*g)*g
-  const float m = __fadd_rn(__fmul_rn(exp_avg[dst], beta1), __fmul_rn(one_minus_beta1, g));
-  const float v = __fadd_rn(__fmul_rn(exp_avg_sq[dst], beta2), __fmul_rn(__fmul_rn(one_minus_beta2, g), g));
-  exp_avg[dst] = m;
-  exp_avg_sq[dst] = v;
-  float vv = v;
-  if (max_exp_avg_sq) { vv = fmaxf(max_exp_avg_sq[dst], v); max_exp_avg_sq[dst] = vv; }
-  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vv), bias_correction2_sqrt), eps);
-  param[dst] = __fadd_rn(param[dst], __fmul_rn(neg_step_size, __fdiv_rn(m, denom)));
+  adam_element(__ldg(grad + t), param + dst, exp_avg + dst, exp_avg_sq + dst, max_exp_avg_sq ? max_exp_avg_sq + dst : nullptr, a);
 }
 
 int launch_sparse_adam(int64_t rows, int C, const int64_t* index, const float* grad, float* param, float* exp_avg,
@@ -38,8 +57,127 @@ int launch_sparse_adam(int64_t rows, int C, const int64_t* index, const float* g
   const int64_t total = rows * C;
   if (total <= 0) return 0;
   const unsigned blocks = (unsigned)((total + ADAM_THREADS - 1) / ADAM_THREADS);
-  sparse_adam_kernel<<<blocks, ADAM_THREADS, 0, st>>>(total, C, index, grad, param, exp_avg, exp_avg_sq, max_exp_avg_sq,
-                                                      beta1, beta2, omb1, omb2, bc2_sqrt, neg_step_size, eps);
+  const AdamConst a{beta1, beta2, omb1, omb2, bc2_sqrt, neg_step_size, eps};
+  sparse_adam_kernel<<<blocks, ADAM_THREADS, 0, st>>>(total, C, index, grad, param, exp_avg, exp_avg_sq, max_exp_avg_sq, a);
+  LGR_CHECK_LAUNCH();
+  return 0;
+}
+
+// ---- LoG's Counter.update_by_output, one view ------------------------------------------------------------------------
+
+// Gaussian of rendered row r: leaves first, then nodes (LoG's torch.cat, counter.py:41-44, level_of_gaussian.py:387-389).
+__device__ __forceinline__ int64_t row_gaussian(int64_t r, int64_t num_leaf, const int64_t* __restrict__ leaf,
+                                                const int64_t* __restrict__ node) {
+  return r < num_leaf ? leaf[r] : node[r - num_leaf];
+}
+
+__device__ __forceinline__ int64_t load_int(const void* p, int64_t j, int bytes) {
+  return bytes == 8 ? static_cast<const int64_t*>(p)[j] : (int64_t) static_cast<const int32_t*>(p)[j];
+}
+
+// torch.norm(grad[:, :2], dim=-1) of one row in fp32: x*x + y*y, each product rounded, then the square root.
+__device__ __forceinline__ float norm2_xy(float x, float y) {
+  return __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
+}
+
+struct CounterArgs {
+  lgr_counter c;
+  int64_t num_leaf, rows, num_points;
+  const int64_t* leaf;
+  const int64_t* node;
+  const int32_t* radii;
+  const float* weight;
+  const float* grad;
+  int64_t gs0, gs1;
+  const void* point_id;
+  const void* point_count;
+  int id_bytes, count_bytes;
+  uint8_t* flag_vis;
+};
+
+__global__ void __launch_bounds__(ADAM_THREADS) counter_update_kernel(const __grid_constant__ CounterArgs a) {
+  const int64_t t = (int64_t)blockIdx.x * ADAM_THREADS + threadIdx.x;
+  if (t < a.rows) {
+    const int32_t radius = a.radii[t];
+    const bool vis = radius > 0;
+    a.flag_vis[t] = vis ? 1 : 0;
+    if (!vis) return;
+    const int64_t g = row_gaussian(t, a.num_leaf, a.leaf, a.node);
+    const float w = a.weight[t];
+    a.c.create_steps_d[g] = (int32_t)((uint32_t)a.c.create_steps_d[g] + 1u);
+    a.c.visible_count_d[g] = (int16_t)(uint16_t)((uint32_t)(uint16_t)a.c.visible_count_d[g] + 1u);
+    const float wm = a.c.weights_max_d[g];
+    a.c.weights_max_d[g] = wm != wm ? wm : w != w ? w : fmaxf(wm, w);      // torch.max: NaN propagates
+    a.c.weights_sum_d[g] = __fadd_rn(a.c.weights_sum_d[g], w);
+    const int16_t r16 = (int16_t)(uint16_t)(uint32_t)radius;
+    const int16_t rm = a.c.radii_max_d[g];
+    a.c.radii_max_d[g] = r16 > rm ? r16 : rm;
+    return;
+  }
+  const int64_t j = t - a.rows;
+  if (j >= a.num_points) return;
+  const int64_t p = load_int(a.point_id, j, a.id_bytes);
+  const int64_t cnt = load_int(a.point_count, j, a.count_bytes);
+  const int64_t g = row_gaussian(p, a.num_leaf, a.leaf, a.node);
+  a.c.area_sum_d[g] = (int32_t)((uint32_t)a.c.area_sum_d[g] + (uint32_t)(uint64_t)cnt);
+  const float n = norm2_xy(a.grad[p * a.gs0], a.grad[p * a.gs0 + a.gs1]);
+  a.c.grad_sum_d[g] = __fadd_rn(a.c.grad_sum_d[g], __fmul_rn(n, (float)cnt));
+  const int32_t c32 = (int32_t)(uint32_t)(uint64_t)cnt;
+  const int32_t rmm = a.c.radii_max_max_d[g];
+  a.c.radii_max_max_d[g] = c32 > rmm ? c32 : rmm;
+}
+
+int launch_counter_update(const lgr_counter& c, int64_t num_leaf, int64_t num_node, const int64_t* leaf,
+                          const int64_t* node, const int32_t* radii, const float* weight, const float* grad,
+                          const int64_t* gs, int64_t num_points, const void* point_id, const void* point_count,
+                          int id_bytes, int count_bytes, uint8_t* flag_vis, cudaStream_t st) {
+  const int64_t rows = num_leaf + num_node, total = rows + num_points;
+  if (total <= 0) return 0;
+  const CounterArgs a{c, num_leaf, rows, num_points, leaf, node, radii, weight, grad, gs[0], gs[1], point_id,
+                      point_count, id_bytes, count_bytes, flag_vis};
+  counter_update_kernel<<<(unsigned)((total + ADAM_THREADS - 1) / ADAM_THREADS), ADAM_THREADS, 0, st>>>(a);
+  LGR_CHECK_LAUNCH();
+  return 0;
+}
+
+// ---- LoG.step: every key's sparse Adam update and the scale clamp, one launch ----------------------------------------
+
+// torch.clamp(v, lo, hi) with tensor bounds: a NaN operand propagates, otherwise min(max(v, lo), hi) (hi where lo > hi).
+__device__ __forceinline__ float torch_clamp(float v, float lo, float hi) {
+  if (v != v) return v;
+  if (lo != lo) return lo;
+  if (hi != hi) return hi;
+  return fminf(fmaxf(v, lo), hi);
+}
+
+__global__ void __launch_bounds__(ADAM_THREADS)
+log_step_kernel(const __grid_constant__ lgr_step s, int64_t num_leaf, int64_t total, const int64_t* __restrict__ leaf,
+                const int64_t* __restrict__ node, const uint8_t* __restrict__ flag_vis) {
+  const int64_t t = (int64_t)blockIdx.x * ADAM_THREADS + threadIdx.x;
+  if (t >= total) return;
+  const int64_t r = t / s.row_floats;
+  if (!flag_vis[r]) return;
+  int col = (int)(t - r * s.row_floats), k = 0;
+  while (k + 1 < s.num_keys && col >= s.keys[k + 1].prefix) k++;
+  const lgr_step_key& key = s.keys[k];
+  col -= key.prefix;
+  const int64_t g = row_gaussian(r, num_leaf, leaf, node);
+  const int64_t dst = g * key.row_floats + col;
+  if (key.grad_d) {
+    const AdamConst a{s.beta1, s.beta2, s.one_minus_beta1, s.one_minus_beta2, key.bc2_sqrt, key.neg_step_size, s.eps};
+    adam_element(__ldg(key.grad_d + r * key.row_floats + col), key.param_d + dst, key.exp_avg_d + dst,
+                 key.exp_avg_sq_d + dst, key.max_exp_avg_sq_d ? key.max_exp_avg_sq_d + dst : nullptr, a);
+  }
+  if (key.clamp)
+    key.param_d[dst] = torch_clamp(key.param_d[dst], logf(s.radius3d_min_d[g]), logf(s.radius3d_max_d[g]));
+}
+
+int launch_log_step(const lgr_step& s, int64_t num_leaf, int64_t num_node, const int64_t* leaf, const int64_t* node,
+                    const uint8_t* flag_vis, cudaStream_t st) {
+  const int64_t total = (num_leaf + num_node) * s.row_floats;
+  if (total <= 0) return 0;
+  log_step_kernel<<<(unsigned)((total + ADAM_THREADS - 1) / ADAM_THREADS), ADAM_THREADS, 0, st>>>(s, num_leaf, total, leaf,
+                                                                                                 node, flag_vis);
   LGR_CHECK_LAUNCH();
   return 0;
 }

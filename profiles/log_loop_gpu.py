@@ -255,6 +255,14 @@ def main():
     rend.ssim_loss = SSIM(11, 3).to(dev)
     res['base_stage_ms_per_iter_fused_ssim'] = T.time(lambda: train_step(model, rend, batch), args.iters)
     rend.ssim_loss = stock_ssim
+    # the same with LoG's post-backward calls on the fused kernels (INTEGRATION.md section 6: Counter.update_by_output
+    # and LoG.step bound to log_b200.optim.counter_update_by_output / log_step)
+    import types
+    from log_b200.optim import counter_update_by_output, log_step
+    model.counter.update_by_output = types.MethodType(counter_update_by_output, model.counter)
+    model.step = types.MethodType(log_step, model)
+    res['base_stage_ms_per_iter_fused_counter_and_step'] = T.time(lambda: train_step(model, rend, batch), args.iters)
+    del model.counter.update_by_output, model.step
 
     # ---- depth stage: LoG's Splitter creates child nodes; every iteration now walks the tree (prepare -> traverse) ----
     model.set_stage('depth')
