@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 22
+#define LGR_ABI_VERSION 23
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -79,6 +79,9 @@ typedef struct lgr_view {
                             slot is taken in lgr_forward_render (two atomic passes over the instances). */
   const int64_t* gather_index_d; /* (n) int64 or NULL (SURVEY 8(f) row 3, the gather of LoG/model/level_of_gaussian.py:262-296
                             fused): the n rows of the call are rows gather_index_d[0..n) of the input TABLES (means3D,
+                            scales, ...); a negative entry is an empty row (radius 0, no table read: it reaches no tile and
+                            its outputs stay as the caller initialised them) -- the device-sized lists of lgr_prepare_cull.
+                            The tables (means3D,
                             scales, rotations, opacities, colors_precomp, shs may hold any number of rows >= max index + 1);
                             every output -- splat, radii, point_weight, point_count, all gradients -- is compact, row i
                             belonging to table row gather_index_d[i], which is exactly the gradient layout LoG's
@@ -343,6 +346,62 @@ int lgr_tree_traverse(const lgr_tree* tree, const float* xyz_d, const float* sca
                       const float* projmatrix_d, const float* viewmatrix_d, float focal_x, float focal_y, float tan_fovx,
                       float tan_fovy, const int64_t* root_index_d, int64_t num_roots, float min_resolution_pixel,
                       int32_t max_depth, int32_t* scratch_d, int64_t* index_out_d, int64_t* count_out_d, void* stream);
+
+/* ---- LoG.prepare (LoG/model/level_of_gaussian.py:223-256; base stage Gaussian.prepare :90-98) --------------------------
+ * The per-view selection of the Gaussians a training step renders, on the device.  Tree mode (num_roots > 0), per view:
+ *   lgr_prepare_cull    root_flag_d[j] = LoG's frustum test of root j (_visible_flag_by_camera, :40-53, in fp32: the
+ *                       four dot products of [x y z 1] with the columns of full_proj_d summed x, y, z, then the constant
+ *                       row; pw = 1 / (w + 1e-7) by IEEE division; p = xyz * pw; 0 < p_z < 1, bound_lo < p_x, p_y <
+ *                       bound_hi); in_range_d (num_roots) = the in-range roots in root order, then -1 up to num_roots
+ *                       (the gather list of the visibility render, see lgr_view.gather_index_d); result_d[IN_RANGE] their
+ *                       number.  LoG renders xyz[root_index][in_range] with scaling[root_index[in_range]], one Gaussian
+ *                       only when root_index[j] == j (TensorTree.initialize): a root whose root_index_d[j] != j counts as
+ *                       out of range and sets result_d[STATUS] = LGR_PREPARE_ROOT_ORDER.
+ *   (the caller renders rows in_range_d of the tables with the fork forward, want_aux, and keeps point_weight and meta_d)
+ *   lgr_prepare_select  root_flag_d[j] = 0 where rendered row k = root j has point_weight_d[k] <= 1e-8; roots_d = the
+ *                       survivors in root order (result_d[ROOTS]); the tree walk of lgr_tree_traverse from them, its
+ *                       root count read on the device (index_all_d, result_d[WALK]); then LoG's leaf / node split of the
+ *                       walk, order-preserving: leaf = (node_index == -1 && depth > 0) with opt_all_levels, else
+ *                       depth == current_depth (leaf_d, node_d; result_d[LEAVES], result_d[NODES]); result_d[INSTANCES]
+ *                       and result_d[OVERFLOW] = meta_d[0] and meta_d[6] of the render (0 with meta_d NULL).
+ * Base stage (num_roots = 0): lgr_prepare_cull alone, over all num_points: flag_d (num_points) and in_range_d = the
+ * flagged ids (result_d[IN_RANGE]).
+ * Nothing synchronises with the host: read result_d (LGR_PREPARE_RESULTS int64) once at the end.  Flag bytes are 0 / 1 (the
+ * bytes of a torch.bool tensor).  scratch_d: LGR_PREPARE_SCRATCH_INTS(num_points, S) int32, S = max(num_roots, num_nodes *
+ * max_child) as for lgr_tree_traverse; num_roots <= num_points. */
+typedef struct lgr_prepare {
+  int64_t num_points, num_roots;
+  const float* xyz_d;          /* (num_points,3) */
+  const float* full_proj_d;    /* (4,4) camera['full_proj_transform'] as LoG multiplies it: [x y z 1] @ M */
+  float bound_lo, bound_hi;    /* fp32(-1 - padding), fp32(1 + padding): LoG's bounds as torch compares them (padding 0.5) */
+  const int32_t* root_index_d; /* (num_roots) TensorTree.root_index */
+  const int32_t* node_index_d; /* (num_points) TensorTree.node_index (select) */
+  const int8_t* depth_d;       /* (num_points) TensorTree.depth (select) */
+  int32_t opt_all_levels, current_depth;
+  uint8_t* flag_d;             /* (num_roots) root_flag, or (num_points) flag */
+  int64_t* in_range_d;         /* (num_roots), or (num_points) index */
+  int64_t* roots_d;            /* (num_roots) */
+  int64_t* index_all_d, *leaf_d, *node_d; /* (num_points) each */
+  int64_t* result_d;           /* (LGR_PREPARE_RESULTS) */
+  int32_t* scratch_d;
+} lgr_prepare;
+#define LGR_PREPARE_RESULTS 8
+#define LGR_PREPARE_IN_RANGE 0
+#define LGR_PREPARE_ROOTS 1
+#define LGR_PREPARE_WALK 2
+#define LGR_PREPARE_LEAVES 3
+#define LGR_PREPARE_NODES 4
+#define LGR_PREPARE_STATUS 5
+#define LGR_PREPARE_INSTANCES 6
+#define LGR_PREPARE_OVERFLOW 7
+#define LGR_PREPARE_ROOT_ORDER 1 /* status: root_index_d[j] != j for some j */
+#define LGR_PREPARE_SCRATCH_INTS(p, s) \
+  (2 * (int64_t)(p) + 2 * (((int64_t)(p) + 255) / 256) + 2 + ((int64_t)(p) + 3) / 4 + LGR_TREE_SCRATCH_INTS(p, s))
+int lgr_prepare_cull(const lgr_prepare* prep, void* stream);
+int lgr_prepare_select(const lgr_prepare* prep, const lgr_tree* tree, const float* scaling_raw_d, const float* rotation_raw_d,
+                       const float* projmatrix_d, const float* viewmatrix_d, float focal_x, float focal_y, float tan_fovx,
+                       float tan_fovy, float min_resolution_pixel, int32_t max_depth, const float* point_weight_d,
+                       const int32_t* meta_d, void* stream);
 
 /* Sorted compaction of the non-zero entries of point_count_d: ids_out_d / counts_out_d (capacity min(N, H*W)) receive the
  * ids in ascending order and their pixel counts, *num_out_d their number.  Equals

@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 22
+LGR_ABI_VERSION = 23
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -22,7 +22,7 @@ EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'l
            'lgr_profile_kernel_name', 'lgr_shard_send', 'lgr_shard_recv_bin', 'lgr_blend_backward', 'lgr_shard_return_rows',
            'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible',
            'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis',
-           'lgr_counter_update', 'lgr_log_step')
+           'lgr_counter_update', 'lgr_log_step', 'lgr_prepare_cull', 'lgr_prepare_select')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -52,6 +52,25 @@ class LgrTree(ctypes.Structure):
 def tree_scratch_ints(num_points, slots):
     """LGR_TREE_SCRATCH_INTS."""
     return 8 + 2 * num_points + slots + 2 * ((slots + 255) // 256) + 2 + (slots + 3) // 4
+
+
+class LgrPrepare(ctypes.Structure):
+    """struct lgr_prepare: LoG.prepare's tables, outputs and scratch."""
+    _fields_ = [('num_points', _i64), ('num_roots', _i64), ('xyz_d', _vp), ('full_proj_d', _vp), ('bound_lo', _f32),
+                ('bound_hi', _f32), ('root_index_d', _vp), ('node_index_d', _vp), ('depth_d', _vp), ('opt_all_levels', _i32),
+                ('current_depth', _i32), ('flag_d', _vp), ('in_range_d', _vp), ('roots_d', _vp), ('index_all_d', _vp),
+                ('leaf_d', _vp), ('node_d', _vp), ('result_d', _vp), ('scratch_d', _vp)]
+
+
+LGR_PREPARE_RESULTS = 8
+(LGR_PREPARE_IN_RANGE, LGR_PREPARE_ROOTS, LGR_PREPARE_WALK, LGR_PREPARE_LEAVES, LGR_PREPARE_NODES, LGR_PREPARE_STATUS,
+ LGR_PREPARE_INSTANCES, LGR_PREPARE_OVERFLOW) = range(8)
+LGR_PREPARE_ROOT_ORDER = 1
+
+
+def prepare_scratch_ints(num_points, slots):
+    """LGR_PREPARE_SCRATCH_INTS."""
+    return 2 * num_points + 2 * ((num_points + 255) // 256) + 2 + (num_points + 3) // 4 + tree_scratch_ints(num_points, slots)
 
 
 LGR_SSIM_WINDOW = 11
@@ -156,6 +175,11 @@ def bind(lib):
     lib.lgr_tree_traverse.restype = ctypes.c_int
     lib.lgr_tree_traverse.argtypes = [ctypes.POINTER(LgrTree), _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _vp, _i64, _f32,
                                       _i32, _vp, _vp, _vp, _vp]
+    lib.lgr_prepare_cull.restype = ctypes.c_int
+    lib.lgr_prepare_cull.argtypes = [ctypes.POINTER(LgrPrepare), _vp]
+    lib.lgr_prepare_select.restype = ctypes.c_int
+    lib.lgr_prepare_select.argtypes = [ctypes.POINTER(LgrPrepare), ctypes.POINTER(LgrTree), _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                       _f32, _i32, _vp, _vp, _vp]
     lib.lgr_ssim_forward.restype = ctypes.c_int
     lib.lgr_ssim_forward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     lib.lgr_ssim_backward.restype = ctypes.c_int

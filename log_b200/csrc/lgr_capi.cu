@@ -37,7 +37,10 @@ int launch_shard_return_packed(const ShardLayout&, const float*, const float*, c
 int launch_shard_return(const ShardLayout&, const float*, int64_t, const void*, int, int64_t, void* const*, cudaStream_t);
 int launch_shard_gather(const View&, const ShardLayout&, int64_t, const float*, const int32_t*, const int32_t*, const float*,
                         float*, float*, int32_t*, int, cudaStream_t);
-int launch_tree_traverse(const TreeArgs&, int64_t, int64_t, const int64_t*, int64_t, int, int32_t*, int64_t*, int64_t*, cudaStream_t);
+int launch_tree_traverse(const TreeArgs&, int64_t, int64_t, const int64_t*, int64_t, const int64_t*, int, int32_t*, int64_t*, int64_t*,
+                         cudaStream_t);
+int launch_prepare_cull(const lgr_prepare&, cudaStream_t);
+int launch_prepare_select(const lgr_prepare&, const TreeArgs&, int64_t, int, const float*, const int32_t*, cudaStream_t);
 int launch_ssim_fwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, double*, float*, float*,
                     cudaStream_t);
 int launch_ssim_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
@@ -507,8 +510,41 @@ int lgr_tree_traverse(const lgr_tree* tree, const float* xyz_d, const float* sca
   a.xyz = xyz_d; a.scaling_raw = scaling_raw_d; a.rotation_raw = rotation_raw_d; a.view = viewmatrix_d; a.proj = projmatrix_d;
   a.fx = focal_x; a.fy = focal_y; a.tanfovx = tan_fovx; a.tanfovy = tan_fovy; a.min_px = min_resolution_pixel;
   const int levels = tree->max_level < max_depth ? tree->max_level : max_depth;
-  return launch_tree_traverse(a, tree->num_points, tree->num_nodes, root_index_d, num_roots, levels, scratch_d, index_out_d,
+  return launch_tree_traverse(a, tree->num_points, tree->num_nodes, root_index_d, num_roots, nullptr, levels, scratch_d, index_out_d,
                               count_out_d, (cudaStream_t)stream);
+}
+
+/* ---- LoG.prepare ---- */
+static bool prepare_ok(const lgr_prepare* p) {
+  if (!p || p->num_points < 0 || p->num_roots < 0 || p->num_roots > p->num_points || !p->result_d) return false;
+  if (p->num_points > 0 && (!p->xyz_d || !p->full_proj_d || !p->flag_d || !p->in_range_d || !p->scratch_d)) return false;
+  if (p->num_roots > 0 && !p->root_index_d) return false;
+  return true;
+}
+
+int lgr_prepare_cull(const lgr_prepare* prep, void* stream) {
+  if (!prepare_ok(prep)) return LGR_E_BADARG;
+  if (prep->num_points > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  return launch_prepare_cull(*prep, (cudaStream_t)stream);
+}
+
+int lgr_prepare_select(const lgr_prepare* prep, const lgr_tree* tree, const float* scaling_raw_d, const float* rotation_raw_d,
+                       const float* projmatrix_d, const float* viewmatrix_d, float focal_x, float focal_y, float tan_fovx,
+                       float tan_fovy, float min_resolution_pixel, int32_t max_depth, const float* point_weight_d,
+                       const int32_t* meta_d, void* stream) {
+  if (!prepare_ok(prep) || prep->num_roots == 0 || !tree || tree->num_points != prep->num_points) return LGR_E_BADARG;
+  if (tree->num_nodes < 0 || tree->max_child <= 0 || tree->max_level < 0 || max_depth < 0) return LGR_E_BADARG;
+  if (!tree->node_index_d || (tree->num_nodes > 0 && !tree->tree_d) || !scaling_raw_d || !rotation_raw_d || !projmatrix_d ||
+      !viewmatrix_d || !point_weight_d || !prep->node_index_d || !prep->depth_d || !prep->roots_d || !prep->index_all_d ||
+      !prep->leaf_d || !prep->node_d)
+    return LGR_E_BADARG;
+  if (tree->num_points > 0x7fffffffLL || tree->num_nodes * tree->max_child > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  TreeArgs a;
+  a.node_index = tree->node_index_d; a.tree = tree->tree_d; a.C = tree->max_child;
+  a.xyz = prep->xyz_d; a.scaling_raw = scaling_raw_d; a.rotation_raw = rotation_raw_d; a.view = viewmatrix_d; a.proj = projmatrix_d;
+  a.fx = focal_x; a.fy = focal_y; a.tanfovx = tan_fovx; a.tanfovy = tan_fovy; a.min_px = min_resolution_pixel;
+  const int levels = tree->max_level < max_depth ? tree->max_level : max_depth;
+  return launch_prepare_select(*prep, a, tree->num_nodes, levels, point_weight_d, meta_d, (cudaStream_t)stream);
 }
 
 /* ---- diagnostics: per-kernel CUDA-event timing (used by bench.py for the live roofline numbers) ---- */

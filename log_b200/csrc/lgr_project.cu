@@ -167,8 +167,13 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
   }
   bool big_splat = false;      // covers more than 4 tiles: counted by the whole warp after the divergent part
   int bx0 = 0, by0 = 0, bx1 = 0, by1 = 0;
-  // gather-fused call (lgr_view.gather_index_d): row i of every output is Gaussian gather[i] of the input tables
-  const int64_t src = (v.gather && work) ? v.gather[i] : i;
+  // gather-fused call (lgr_view.gather_index_d): row i of every output is Gaussian gather[i] of the input tables; a
+  // negative entry is an empty row (radius 0, no table read)
+  int64_t src = i;
+  if (v.gather && work) {
+    src = v.gather[i];
+    if (src < 0) work = false;
+  }
   if (work) {
     float p[3], Sg[9];
     load3(means, src, p);

@@ -166,21 +166,24 @@ __global__ void tree_finish_kernel(int32_t* __restrict__ state, int64_t* __restr
   *count_out = state[ST_OUT];
 }
 
-__global__ void tree_init_kernel(int32_t* __restrict__ state, int num_roots) {
-  state[ST_FRONT] = num_roots; state[ST_OUT] = 0; state[2] = 0; state[3] = 0;
+// num_roots_d: the root count on the device (the walk of lgr_prepare_select), else num_roots
+__global__ void tree_init_kernel(int32_t* __restrict__ state, int num_roots, const int64_t* __restrict__ num_roots_d) {
+  state[ST_FRONT] = num_roots_d ? (int)*num_roots_d : num_roots; state[ST_OUT] = 0; state[2] = 0; state[3] = 0;
 }
 
 // scratch layout (int32 units): state[8] | front A [P] | front B [P] | cand [S] | chunk counts [2 * ceil(S/256) + 2] |
-// flags [S bytes], with P = num_points, S = max(num_roots, num_nodes * C) candidate slots of one level
+// flags [S bytes], with P = num_points, S = max(num_roots, num_nodes * C) candidate slots of one level.  num_roots_d: the
+// number of roots lives on the device (at most num_roots, which then only sizes the scratch).
 int launch_tree_traverse(const TreeArgs& a, int64_t num_points, int64_t num_nodes, const int64_t* roots, int64_t num_roots,
-                         int levels, int32_t* scratch, int64_t* out, int64_t* count_out, cudaStream_t st) {
+                         const int64_t* num_roots_d, int levels, int32_t* scratch, int64_t* out, int64_t* count_out,
+                         cudaStream_t st) {
   const int64_t S = num_roots > num_nodes * a.C ? num_roots : num_nodes * a.C;
   int32_t* state = scratch;
   int32_t* front[2] = {scratch + 8, scratch + 8 + num_points};
   int32_t* cand = scratch + 8 + 2 * num_points;
   int32_t* chunk_cnt = cand + S;
   uint8_t* flags = reinterpret_cast<uint8_t*>(chunk_cnt + 2 * ((S + TREE_THREADS - 1) / TREE_THREADS) + 2);
-  tree_init_kernel<<<1, 1, 0, st>>>(state, (int)num_roots);
+  tree_init_kernel<<<1, 1, 0, st>>>(state, (int)num_roots, num_roots_d);
   LGR_CHECK_LAUNCH();
   // level 0: the roots themselves
   tree_classify_kernel<true><<<TREE_GRID, TREE_THREADS, 0, st>>>(a, roots, nullptr, state, cand, flags, chunk_cnt);

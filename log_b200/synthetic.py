@@ -89,3 +89,52 @@ def make_scene(n, width, height, median_radius_px, seed=0, sh_degree=0, fovx_deg
 def make_cotangent(channels, height, width, seed=1, dtype=torch.float64):
     g = torch.Generator().manual_seed(seed)
     return torch.randn(channels, height, width, generator=g, dtype=torch.float64).to(dtype)
+
+
+def make_log_forest(num_roots, levels, width, height, seed=0, max_child=2, p_split=0.55, fovx_deg=60.0, zfar=100.0):
+    """Seeded level-of-Gaussian forest as LoG's TensorTree stores it, for the camera of make_camera(width, height): roots
+    0..R-1 (TensorTree.initialize), children appended level by level; per level a node splits with probability p_split,
+    and each child slot stays empty (-1, as after LoG's removals) with probability 0.15.  Roots lie in view depth
+    (0.5, 30), 2 % behind the camera and 2 % past the far plane, NDC x, y in (-2, 2); 1 sigma is 1..8 pixels, halving per
+    level; 10 % of the opacity logits are -9 (composite nothing).  Returns a dict of float64 / int tensors: xyz,
+    scaling (log-scales), rotation (raw), opacity (N,1) logits, colors, and root_index / node_index / tree int32, depth int8."""
+    g = torch.Generator().manual_seed(seed)
+    u = lambda *s: torch.rand(*s, generator=g, dtype=torch.float64)
+    R = int(num_roots)
+    tanx = math.tan(math.radians(fovx_deg) * 0.5)
+    fx = width / (2 * tanx)
+    tany = height / (2 * fx)
+    z = 0.5 + 29.5 * u(R)
+    k = R // 50
+    z[:k] = -0.1 - 5.0 * u(k)
+    z[k:2 * k] = zfar + 0.5 + 20.0 * u(k)
+    xyz = torch.stack([(4 * u(R) - 2) * z * tanx, (4 * u(R) - 2) * z * tany, z], -1)
+    sig = (1.0 + 7.0 * u(R)) * z.abs() / fx
+    xyzs, sigs, depths, rows = [xyz], [sig], [torch.zeros(R, dtype=torch.int8)], []
+    frontier, count = torch.arange(R), R
+    for level in range(1, levels + 1):
+        has = frontier[u(frontier.numel()) < p_split]
+        keep = u(has.numel(), max_child) >= 0.15
+        keep[:, 0] = True
+        ids = torch.cumsum(keep.reshape(-1).long(), 0).reshape(keep.shape) - 1 + count
+        table = torch.where(keep, ids, torch.full_like(ids, -1)).to(torch.int32)
+        parent = has[:, None].expand_as(keep)[keep]
+        n_new = int(parent.numel())
+        rows.append((has, table))
+        xyzs.append(torch.cat(xyzs)[parent] + torch.randn(n_new, 3, generator=g, dtype=torch.float64) * torch.cat(sigs)[parent, None])
+        sigs.append(torch.cat(sigs)[parent] * 0.5)
+        depths.append(torch.full((n_new,), level, dtype=torch.int8))
+        frontier, count = torch.arange(count, count + n_new), count + n_new
+    ni = torch.full((count,), -1, dtype=torch.int32)
+    table = torch.cat([t for _, t in rows]) if rows else torch.zeros((0, max_child), dtype=torch.int32)
+    m = 0
+    for has, _ in rows:
+        ni[has] = torch.arange(m, m + has.numel(), dtype=torch.int32)
+        m += has.numel()
+    xyz, sig = torch.cat(xyzs), torch.cat(sigs)
+    N = xyz.shape[0]
+    scaling = torch.log(sig[:, None] * (0.5 + 0.5 * u(N, 3)))
+    opacity = 2.0 * torch.randn(N, 1, generator=g, dtype=torch.float64)
+    opacity[u(N) < 0.1] = -9.0
+    return dict(xyz=xyz, scaling=scaling, rotation=torch.randn(N, 4, generator=g, dtype=torch.float64), opacity=opacity,
+                colors=u(N, 3), root_index=torch.arange(R, dtype=torch.int32), node_index=ni, tree=table, depth=torch.cat(depths))

@@ -278,6 +278,12 @@ def main():
     model.optimizer.step = fused_adam_step(model)
     res['depth_stage_ms_per_iter_fused_walk_and_adam'] = T.time(lambda: train_step(model, rend, batch), args.iters)
     model.optimizer.step = stock_step
+    # the same with LoG.prepare bound to log_b200.prepare.log_prepare (INTEGRATION.md section 6): cull, visibility render,
+    # walk and leaf / node split with one host read per view.  Not measured yet: it needs a LoG checkout.
+    from log_b200.prepare import log_prepare
+    model.prepare = types.MethodType(log_prepare, model)
+    res['depth_stage_ms_per_iter_fused_prepare'] = T.time(lambda: train_step(model, rend, batch), args.iters)
+    del model.prepare
 
     # ---- rows in isolation on this model state ----
     camera, rasterizer, _ = rend.prepare_camera(batch, 0, None, is_train=True)      # renderer.py:207-223, as vis() does
