@@ -513,9 +513,12 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     const float o = act_sigmoid(__ldg(opac + src));
     dop *= o * (1.0f - o);                                                        // d sigmoid = o (1 - o)
     float inv;
-    const float4 qn = act_normalize(ldg4(rots + 4 * src), inv);
-    const float dot = qn.x * dq[0] + qn.y * dq[1] + qn.z * dq[2] + qn.w * dq[3];
-    dq[0] = (dq[0] - qn.x * dot) * inv; dq[1] = (dq[1] - qn.y * dot) * inv;       // d (r/|r|) = (I - q q^T) / |r|
+    const float4 qr = ldg4(rots + 4 * src);
+    const float4 qn = act_normalize(qr, inv);
+    // d (r / max(|r|, eps)) = (I - q q^T) / |r|, and I / eps below eps (F.normalize: the max is a constant there)
+    const bool below = sqrtf(qr.x * qr.x + qr.y * qr.y + qr.z * qr.z + qr.w * qr.w) < 1e-12f;
+    const float dot = below ? 0.f : qn.x * dq[0] + qn.y * dq[1] + qn.z * dq[2] + qn.w * dq[3];
+    dq[0] = (dq[0] - qn.x * dot) * inv; dq[1] = (dq[1] - qn.y * dot) * inv;
     dq[2] = (dq[2] - qn.z * dot) * inv; dq[3] = (dq[3] - qn.w * dot) * inv;
     if (LOG_SH) {      // d rest_k = B_k(dir) * d rgb ; the direction is detached (activation.py:30): nothing flows to the mean
       float* dsh = dshs + (int64_t)i * K * 3;
