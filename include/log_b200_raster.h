@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 23
+#define LGR_ABI_VERSION 24
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -71,12 +71,8 @@ typedef struct lgr_view {
   float* band_dsplat_d;  /* (N,12) or NULL: the backward's dsplat_d; lgr_forward_render zeroes the rows of listed
                             Gaussians so that the caller need not zero-fill all N rows.  Also honoured with num_owners = 0:
                             the rows of all Gaussians with radius > 0 are zeroed (the only rows lgr_backward reads) */
-  int32_t* tile_rank_d;  /* (rows,4) int32 or NULL.  When set, the counting pass (lgr_forward_project / lgr_shard_recv_bin)
-                            takes the tile slots of every splat that covers <= 4 tiles with RETURNING atomics and stores
-                            the 4 ranks here (row = Gaussian index); lgr_forward_render then places those instances at
-                            tile_start + rank without touching an atomic again.  Splats covering more tiles are counted
-                            in a second per-tile counter and still take their slots in lgr_forward_render.  NULL: every
-                            slot is taken in lgr_forward_render (two atomic passes over the instances). */
+  int32_t* tile_rank_d;  /* ignored (kept for the layout): the counting pass no longer takes tile slots, the binning of
+                            lgr_forward_render takes them itself */
   const int64_t* gather_index_d; /* (n) int64 or NULL (SURVEY 8(f) row 3, the gather of LoG/model/level_of_gaussian.py:262-296
                             fused): the n rows of the call are rows gather_index_d[0..n) of the input TABLES (means3D,
                             scales, ...); a negative entry is an empty row (radius 0, no table read: it reaches no tile and
@@ -182,8 +178,8 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
 
 /* Stage 2 of the forward: bin (Gaussian,tile) instances, per-tile (depth,index) radix sort, front-to-back blend.
  *   num_instances / max_tile_len / num_long_tiles : the values read from meta_d[0], meta_d[1], meta_d[5]
- *   scratch: inst_key_d, inst_val_d (num_instances) uint32; inst_tmp_d (2*num_instances) uint32, only needed when
- *            max_tile_len exceeds the shared-memory sort capacity (lgr_sort_smem_capacity()), else may be NULL
+ *   scratch: inst_key_d, inst_val_d (num_instances) uint32; inst_tmp_d (2*num_instances) uint32, 8-byte aligned: the
+ *            binning's staging buffer (and the sort's scratch for lists longer than lgr_sort_smem_capacity())
  *   out: sorted_ids_d (num_instances) int32 (kept for backward); image_d (3,H,W) (6,H,W with num_channels = 6); final_T_d (H,W);
  *        n_contrib_d (H,W) int32; when view->want_aux: point_id_pixel_d (H,W) int32, point_weight_pixel_d (H,W),
  *        point_weight_d (N) -- must be zero-filled by the caller;
@@ -200,7 +196,8 @@ int32_t lgr_sort_smem_capacity(void);
 /* Stage 2 without the host read of meta_d ("device-sized"): the same work as lgr_forward_render, but every launch shape is
  * independent of D / the longest list / the number of long tiles -- the kernels read them from meta_d on the device -- so the
  * whole forward needs no host synchronisation and can be captured in a CUDA graph.  The caller sizes inst_key_d /
- * inst_val_d / sorted_ids_d for `instance_capacity` instances (e.g. 1.25 x the D of the previous view).  If the view needs
+ * inst_val_d / sorted_ids_d for `instance_capacity` instances (e.g. 1.25 x the D of the previous view), inst_tmp_d for
+ * 2 x instance_capacity (the binning's staging buffer, 8-byte aligned).  If the view needs
  * more (meta_d[0] > instance_capacity) or holds a tile list longer than lgr_sort_smem_capacity(), nothing is written out of
  * bounds, meta_d[6] is set to a non-zero value (bit 0: capacity, bit 1: list too long) and the outputs of this view are
  * INVALID: the caller checks meta_d[6] when it next synchronises and redoes the view through lgr_forward_render.
@@ -208,7 +205,7 @@ int32_t lgr_sort_smem_capacity(void);
 int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t instance_capacity, int32_t* meta_d,
                                     const float* splat_d, const int32_t* radii_d, int32_t* tile_start_d,
                                     int32_t* tile_cursor_d, uint32_t* inst_key_d, uint32_t* inst_val_d,
-                                    int32_t* sorted_ids_d, float* image_d, float* final_T_d, int32_t* n_contrib_d,
+                                    uint32_t* inst_tmp_d, int32_t* sorted_ids_d, float* image_d, float* final_T_d, int32_t* n_contrib_d,
                                     int32_t* point_id_pixel_d, float* point_weight_pixel_d, float* point_weight_d,
                                     int32_t* point_count_d, void* stream);
 

@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 23
+LGR_ABI_VERSION = 24
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -143,7 +143,7 @@ def bind(lib):
     lib.lgr_forward_render.restype = ctypes.c_int
     lib.lgr_forward_render.argtypes = [ctypes.POINTER(LgrView), _i64, _i64, _i32, _i32] + [_vp] * 16
     lib.lgr_forward_render_device_sized.restype = ctypes.c_int
-    lib.lgr_forward_render_device_sized.argtypes = [ctypes.POINTER(LgrView), _i64, _i64] + [_vp] * 16
+    lib.lgr_forward_render_device_sized.argtypes = [ctypes.POINTER(LgrView), _i64, _i64] + [_vp] * 17
     lib.lgr_sparse_adam.restype = ctypes.c_int
     lib.lgr_sparse_adam.argtypes = [_i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, ctypes.c_double, ctypes.c_double,
                                     ctypes.c_double, ctypes.c_double, _vp]

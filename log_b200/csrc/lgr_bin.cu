@@ -1,8 +1,8 @@
-// Tile binning: exclusive scan of the per-tile counts, scatter of (depth, id) instances into per-tile bins,
-// and the per-tile sort by (depth, id).
+// Tile binning: exclusive scan of the per-tile counts, placement of the (depth, id) instances into per-tile bins (two
+// passes, grouped by tile row first), and the per-tile sort by (depth, id).
 //
 // Design: instead of one global 64-bit key sort over all D instances (6+ passes x 24 B/instance through
-// HBM), instances are counting-sorted into tile bins (one 8-byte scattered write each) and every tile's list is
+// HBM), instances are counting-sorted into tile bins (staged by tile row, then placed) and every tile's list is
 // then sorted entirely in shared memory by one CTA (one 8-byte read + one 4-byte write per instance): an MSD bucket
 // partition on the highest differing bits of the unique (depth, id) composite, finished by rank counting inside the
 // buckets.  Lists that do not fit the 227 KB of shared memory take a stable LSD radix sort over global scratch.
@@ -20,10 +20,11 @@ constexpr int SORT_CAP_SMALL_FWD = 4096;   // lists up to this length are sorted
 
 __global__ void __launch_bounds__(SCAN_THREADS)
 tile_scan_kernel(int ntiles, int32_t* __restrict__ tile_start /* out: starts[0..ntiles] */,
-                 int32_t* __restrict__ cursor /* [0,CSTRIDE*ntiles): per tile [0] = small-splat count, [1] = big-splat count
-                                                 in; out: ranked ? ([0] kept = offset of the big splats, [1] = 0 their
-                                                 cursor) : ([0] = 0 the cursor) ; then ntiles ints: ids of long tiles */,
-                 int32_t* __restrict__ meta, int small_cap, int ranked) {
+                 int32_t* __restrict__ cursor /* [0,CSTRIDE*ntiles): per tile [0] + [1] = its count in; out: [0] = 0 the
+                                                 tile's cursor for bin_place ([2] of a row's first tile, the row's cursor
+                                                 for bin_partition, is never counted into: zero from the entry point's
+                                                 memset) ; then ntiles ints: ids of long tiles */,
+                 int32_t* __restrict__ meta, int small_cap) {
   __shared__ int warp_sum[SCAN_THREADS / 32];
   __shared__ int carry_s, maxl_s, nbig_s;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -49,7 +50,7 @@ tile_scan_kernel(int ntiles, int32_t* __restrict__ tile_start /* out: starts[0..
     const int carry = carry_s;
     const int excl = carry + (wid ? warp_sum[wid - 1] : 0) + x - c;
     if (i < ntiles) {
-      tile_start[i] = excl; cursor[i * CSTRIDE + ranked] = 0;
+      tile_start[i] = excl; cursor[i * CSTRIDE] = 0;
       if (c > small_cap) cursor[CSTRIDE * ntiles + atomicAdd(&nbig_s, 1)] = i;   // tiles the main sort launch cannot hold
     }
     __syncthreads();
@@ -64,105 +65,309 @@ tile_scan_kernel(int ntiles, int32_t* __restrict__ tile_start /* out: starts[0..
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// scatter instances into tile bins (order inside a bin is arbitrary; the sort fixes it)
+// binning in two passes (order inside a bin is arbitrary; the sort fixes it)
 // ---------------------------------------------------------------------------------------------------------
-constexpr int SCATTER_THREADS = 256;
+// The instances of a tile are stored at tile_start[t] + rank, and the Gaussians arrive in random memory order: stored
+// straight to their tiles, the 8 stores that fill one 32-byte sector of a list arrive at random times across the whole
+// kernel, the lists are larger than L2, and most sectors are written back half filled.  So the stores are reordered in
+// time instead:
+//   bin_partition: a CTA bins a chunk of Gaussians, groups the instances by tile ROW in shared memory and writes each row's
+//     group as one contiguous run (reserved with one atomic on a per-row cursor) into a staging buffer.  Row r's region of
+//     it is [tile_start[r*gx], tile_start[(r+1)*gx]): tile_start is a row-major scan, so no other scan is needed.  A staged
+//     instance is the (depth key, id) composite in `stage` and its tile in `stage_tile`.
+//   bin_place: CTAs read the staging buffer in order, i.e. tile row by tile row, and place each instance at tile_start[t] +
+//     a per-tile cursor (counted in shared memory, one global atomic per tile and CTA).  Only a few rows are in flight at a
+//     time, and one row's lists (a few MB) stay in L2 until their sectors are complete.
+constexpr int BIN_THREADS = 256;
+constexpr int PART_ROUNDS = 8;                       // bin_partition: a CTA's chunk is up to PART_ROUNDS x 256 Gaussians
+// bin_place: CTAs in flight, striding over the chunks in staging order; 4 per SM of the H100's 132 (on the 10 M workload
+// 2 or 6 per SM were slower: 0.42 / 0.37 ms against 0.31)
+constexpr int PLACE_GRID = 132 * 4;
+constexpr int PART_CAP = 2048;                       // small-splat instances held in shared memory between two flushes
+constexpr int PART_FLUSH_AT = PART_CAP - 4 * BIN_THREADS;      // a round adds at most 4 per Gaussian
+constexpr int PLACE_ITEMS = 8;
+constexpr int PLACE_CHUNK = PLACE_ITEMS * BIN_THREADS;         // bin_place: staged instances per CTA
+#ifndef LGR_BIN_DIRECT_MAX
+#define LGR_BIN_DIRECT_MAX (1 << 16)      // the CPU emulation's tests also build with 0, to take the two passes on small views
+#endif
+constexpr int64_t BIN_DIRECT_MAX = LGR_BIN_DIRECT_MAX;      // views of at most this many instances: bin_partition places them itself
+constexpr int PLACE_WINDOW = 2047;                   // tiles (from the first row of a chunk on) whose cursors are counted in shared memory
 
-__global__ void __launch_bounds__(SCATTER_THREADS)
-bin_scatter_kernel(View v, int64_t n, const float* __restrict__ splat, const int32_t* __restrict__ radii,
-                   const int32_t* __restrict__ tile_start, int32_t* __restrict__ cursor, uint32_t* __restrict__ inst_key,
-                   uint32_t* __restrict__ inst_val, int64_t capacity /* of inst_key / inst_val: stores beyond it are dropped */) {
-  // No early return: big splats are scattered by the whole warp below (convergent ballots / shuffles).
+__device__ __forceinline__ unsigned long long composite(uint32_t k, uint32_t v) { return ((unsigned long long)k << 32) | v; }
+
+int part_smem_bytes(int rows) { return 3 * (int)sizeof(int32_t) * max(rows, 1); }
+
+// Exclusive scan of in[0,len) into out (in == out allowed).  Block-wide, convergent; `wsum` holds BIN_THREADS/32 ints.
+__device__ __forceinline__ void block_exclusive_scan(const int* in, int* out, int len, int* wsum) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  int carry = 0;
+  for (int base = 0; base < len; base += BIN_THREADS) {
+    const int c = base + tid < len ? in[base + tid] : 0;
+    int x = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) wsum[wid] = x;
+    __syncthreads();
+    int before = carry, all = carry;
+#pragma unroll
+    for (int w = 0; w < BIN_THREADS / 32; w++) { if (w < wid) before += wsum[w]; all += wsum[w]; }
+    if (base + tid < len) out[base + tid] = before + x - c;
+    carry = all;
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(BIN_THREADS, 6)
+bin_partition_kernel(View v, int64_t n, const float* __restrict__ splat, const int32_t* __restrict__ radii,
+                     const int32_t* __restrict__ tile_start, int32_t* __restrict__ cursor, unsigned long long* __restrict__ stage,
+                     int32_t* __restrict__ stage_tile, int64_t capacity /* of the staging buffer: stores beyond it are dropped */,
+                     int rounds /* chunk = rounds x 256 Gaussians, 1..PART_ROUNDS */,
+                     uint32_t* __restrict__ direct_key, uint32_t* __restrict__ direct_val /* non-NULL: small view, place the
+                     instances into these lists directly (one returning atomic each), no staging */) {
+  // No early return: big splats are walked by the whole warp, and the flushes are block-wide.
   // Shard mode (View::region_count): the kernel strides over the USED rows only; otherwise the grid covers the n rows and
-  // the loop runs once.
+  // the chunk loop runs once.
+  extern __shared__ int32_t row_tab[];      // per tile row: [0,rows) instances held, [rows,2rows) their offset, [2rows,3rows) run base
+  __shared__ uint32_t s_key[PART_CAP], s_id[PART_CAP];
+  __shared__ int32_t s_tile[PART_CAP];
+  __shared__ uint16_t s_perm[PART_CAP];
+  __shared__ int s_fill;
+  __shared__ int s_wsum[BIN_THREADS / 32];
   __shared__ int64_t s_first[LGR_SHARD_MAX_RANKS + 1];
-  const int64_t total = v.region_count ? region_setup(v, s_first) : n;
-  for (int64_t base = (int64_t)blockIdx.x * SCATTER_THREADS; base < total; base += (int64_t)gridDim.x * SCATTER_THREADS) {
-  int64_t i = base + threadIdx.x;
-  bool live = i < total;
-  if (live && v.region_count) i = region_row(v, s_first, i);
-  if (live && v.num_owners > 0) {      // band mode: slot i of the per-CTA id lists written by project_fwd (256 ids per CTA)
-    const int b = (int)(i / 256), sl = (int)(i % 256);
-    if (sl >= v.band_blk[b]) live = false;
-    else {
-      const int id = v.band_ids[i];
-      v.band_rows[v.band_blk[v.band_blocks + b] + sl] = id;      // dense packed-row -> id map for the backward
-      if (v.band_dsplat) {                                       // the sweep's accumulators: zero only the listed rows
-        float4* z = reinterpret_cast<float4*>(v.band_dsplat + (int64_t)id * LGR_GRAD_FLOATS);
+  const int rows = v.row1 - v.row0, lane = threadIdx.x & 31;
+  int32_t* r_cnt = row_tab;
+  int32_t* r_off = row_tab + rows;
+  int32_t* r_base = row_tab + 2 * rows;
+  for (int r = threadIdx.x; r < rows; r += BIN_THREADS) r_cnt[r] = 0;
+  if (threadIdx.x == 0) s_fill = 0;
+  const int64_t total = v.region_count ? region_setup(v, s_first) : n;      // region_setup: a barrier
+  __syncthreads();
+  // Writes the held instances out, one run per non-empty tile row, and empties the buffer.  Block-wide.
+  auto flush = [&]() {
+    const int held = s_fill;
+    if (direct_key) {      // the lists fit in L2: no second pass
+      for (int e = threadIdx.x; e < held; e += BIN_THREADS) {
+        const int t = s_tile[e];
+        const int64_t pos = (int64_t)tile_start[t] + atomicAdd(cursor + t * CSTRIDE, 1);
+        if (pos < capacity) { direct_key[pos] = s_key[e]; direct_val[pos] = s_id[e]; }
+      }
+      __syncthreads();
+      for (int r = threadIdx.x; r < rows; r += BIN_THREADS) r_cnt[r] = 0;
+      if (threadIdx.x == 0) s_fill = 0;
+      __syncthreads();
+      return;
+    }
+    for (int r = threadIdx.x; r < rows; r += BIN_THREADS) {
+      const int c = r_cnt[r];
+      if (c > 0) r_base[r] = tile_start[r * v.gx] + atomicAdd(cursor + r * v.gx * CSTRIDE + 2, c);
+    }
+    block_exclusive_scan(r_cnt, r_off, rows, s_wsum);
+    for (int r = threadIdx.x; r < rows; r += BIN_THREADS) r_base[r] -= r_off[r];      // run base minus the group's offset
+    __syncthreads();
+    for (int e = threadIdx.x; e < held; e += BIN_THREADS) s_perm[atomicAdd(&r_off[s_tile[e] / v.gx], 1)] = (uint16_t)e;
+    __syncthreads();
+    for (int j = threadIdx.x; j < held; j += BIN_THREADS) {      // consecutive j: consecutive positions of one run
+      const int e = s_perm[j], t = s_tile[e];
+      const int64_t pos = (int64_t)r_base[t / v.gx] + j;
+      if (pos < capacity) { stage[pos] = composite(s_key[e], s_id[e]); stage_tile[pos] = t; }
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < rows; r += BIN_THREADS) r_cnt[r] = 0;
+    if (threadIdx.x == 0) s_fill = 0;
+    __syncthreads();
+  };
+  for (int64_t chunk = (int64_t)blockIdx.x * rounds * BIN_THREADS; chunk < total; chunk += (int64_t)gridDim.x * rounds * BIN_THREADS) {
+    for (int round = 0; round < rounds; round++) {
+      int64_t i = chunk + round * BIN_THREADS + threadIdx.x;
+      bool live = i < total;
+      if (live && v.region_count) i = region_row(v, s_first, i);
+      if (live && v.num_owners > 0) {      // band mode: slot i of the per-CTA id lists written by project_fwd (256 ids per CTA)
+        const int b = (int)(i / 256), sl = (int)(i % 256);
+        if (sl >= v.band_blk[b]) live = false;
+        else {
+          const int id = v.band_ids[i];
+          v.band_rows[v.band_blk[v.band_blocks + b] + sl] = id;      // dense packed-row -> id map for the backward
+          if (v.band_dsplat) {                                       // the sweep's accumulators: zero only the listed rows
+            float4* z = reinterpret_cast<float4*>(v.band_dsplat + (int64_t)id * LGR_GRAD_FLOATS);
+            z[0] = z[1] = z[2] = make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+          i = id;
+        }
+      }
+      // All per-Gaussian loads are issued together, before anything depends on them (radius, the two record quads with
+      // the depth): one memory latency instead of a chain.  Nearly every row is live, so nothing is wasted.
+      int rad = 0;
+      float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0;
+      float depth = 0.f;
+      if (live) {
+        rad = radii[i];
+        r0 = ldg4(splat + i * LGR_SPLAT_FLOATS);
+        r1 = ldg4(splat + i * LGR_SPLAT_FLOATS + 4);
+        depth = __ldg(splat + i * LGR_SPLAT_FLOATS + 11);
+        live = rad > 0;
+      }
+      if (live && v.num_owners == 0 && v.band_dsplat) {      // optional: zero the backward's accumulator row of every visible Gaussian here,
+        float4* z = reinterpret_cast<float4*>(v.band_dsplat + i * LGR_GRAD_FLOATS);      // instead of a separate full-size memset
         z[0] = z[1] = z[2] = make_float4(0.f, 0.f, 0.f, 0.f);
       }
-      i = id;
-    }
-  }
-  // All per-Gaussian loads are issued together, before anything depends on them (radius, the two record quads with the
-  // depth, the four ranks): one memory latency instead of a chain of three.  Nearly every row is live, so nothing is wasted.
-  int rad = 0;
-  float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0;
-  float depth = 0.f;
-  int4 rk = make_int4(-1, -1, -1, -1);
-  if (live) {
-    rad = radii[i];
-    r0 = ldg4(splat + i * LGR_SPLAT_FLOATS);
-    r1 = ldg4(splat + i * LGR_SPLAT_FLOATS + 4);
-    depth = __ldg(splat + i * LGR_SPLAT_FLOATS + 11);
-    if (v.tile_rank) rk = __ldg(reinterpret_cast<const int4*>(v.tile_rank + 4 * i));
-    live = rad > 0;
-  }
-  if (live && v.num_owners == 0 && v.band_dsplat) {      // optional: zero the backward's accumulator row of every visible Gaussian here,
-    float4* z = reinterpret_cast<float4*>(v.band_dsplat + i * LGR_GRAD_FLOATS);      // instead of a separate full-size memset
-    z[0] = z[1] = z[2] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-  uint32_t key = 0;
-  if (live) {
-    live = r1.z > 0.f;      // hx == 0: opacity below 1/255, contributes nowhere
-    if (live) {
-      key = __float_as_uint(depth);   // depth > 0.2 : IEEE bits are order preserving
-      tile_rect_tight(r0.x, r0.y, rad, r1.z, r1.w, v.gx, v.gy, v.row0, v.row1, x0, y0, x1, y1);
-    }
-  }
-  const int w = x1 - x0, cnt = live ? w * (y1 - y0) : 0;
-  if (cnt > 0 && cnt <= 4) {
-    int t[4], slot[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      const int ty = y0 + k / max(w, 1), tx = x0 + k % max(w, 1);
-      t[k] = k < cnt ? (ty - v.row0) * v.gx + tx : -1;
-    }
-    if (v.tile_rank) {      // the counting pass already took the slots: a streaming kernel, no atomics
-      slot[0] = rk.x; slot[1] = rk.y; slot[2] = rk.z; slot[3] = rk.w;
-    } else {
-      // all slot requests are issued before any dependent store, so the returning atomics overlap instead of forming a
-      // serial chain of L2 round trips
-#pragma unroll
-      for (int k = 0; k < 4; k++) slot[k] = t[k] >= 0 ? atomicAdd(cursor + t[k] * CSTRIDE, 1) : 0;
-    }
-#pragma unroll
-    for (int k = 0; k < 4; k++)
-      if (t[k] >= 0) {
-        const int pos = __ldg(tile_start + t[k]) + slot[k];
-        if (pos < capacity) { inst_key[pos] = key; inst_val[pos] = (uint32_t)i; }
+      int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
+      uint32_t key = 0;
+      if (live) {
+        live = r1.z > 0.f;      // hx == 0: opacity below 1/255, contributes nowhere
+        if (live) {
+          key = __float_as_uint(depth);   // depth > 0.2 : IEEE bits are order preserving
+          tile_rect_tight(r0.x, r0.y, rad, r1.z, r1.w, v.gx, v.gy, v.row0, v.row1, x0, y0, x1, y1);
+        }
       }
-  }
-  // Big splats (more than 4 tiles), one at a time by the whole warp: lane l takes tiles l, l+32, ... of the rectangle, so a
-  // splat covering hundreds of tiles costs a few rounds of overlapping atomics instead of a serial chain in one lane.
-  // ranked: they sit behind the cursor[t][0] small splats of the tile and take their slots from cursor[t][1].
-  const int lane = threadIdx.x & 31, big = v.tile_rank ? 1 : 0;
-  unsigned todo = __ballot_sync(0xffffffffu, cnt > 4);
-  while (todo) {
-    const int src = __ffs(todo) - 1;
-    todo &= todo - 1;
-    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-    const int bw = __shfl_sync(0xffffffffu, w, src), bcnt = __shfl_sync(0xffffffffu, cnt, src);
-    const uint32_t bkey = __shfl_sync(0xffffffffu, key, src);
-    const uint32_t bid = (uint32_t)__shfl_sync(0xffffffffu, (int)i, src);
-    for (int k = lane; k < bcnt; k += 32) {
-      const int t = (by0 + k / bw - v.row0) * v.gx + bx0 + k % bw;
-      const int pos = tile_start[t] + (big ? cursor[t * CSTRIDE] : 0) + atomicAdd(cursor + t * CSTRIDE + big, 1);
-      if (pos < capacity) { inst_key[pos] = bkey; inst_val[pos] = bid; }
+      const int w = x1 - x0, cnt = live ? w * (y1 - y0) : 0;
+      // Small splats (at most 4 tiles): held in shared memory, slots handed out per warp (one shared atomic per warp).
+      const int mine = cnt <= 4 ? cnt : 0;
+      int incl = mine;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += y; }
+      int wbase = 0;
+      if (lane == 31 && incl > 0) wbase = atomicAdd(&s_fill, incl);
+      wbase = __shfl_sync(0xffffffffu, wbase, 31);
+      for (int k = 0, s = wbase + incl - mine; k < mine; k++, s++) {
+        const int ty = y0 + k / w, tx = x0 + k % w;
+        s_key[s] = key; s_id[s] = (uint32_t)i; s_tile[s] = (ty - v.row0) * v.gx + tx;
+        atomicAdd(&r_cnt[ty - v.row0], 1);
+      }
+      // Big splats (more than 4 tiles), one at a time by the whole warp: one run per covered row, reserved by lane l for row
+      // l (the atomics of up to 32 rows overlap), then the lanes fill the runs.
+      unsigned todo = __ballot_sync(0xffffffffu, cnt > 4);
+      while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
+        const int bw = __shfl_sync(0xffffffffu, w, src), bcnt = __shfl_sync(0xffffffffu, cnt, src);
+        const uint32_t bkey = __shfl_sync(0xffffffffu, key, src);
+        const uint32_t bid = (uint32_t)__shfl_sync(0xffffffffu, (int)i, src);
+        const int bh = bcnt / bw;
+        if (direct_key) {
+          for (int k = lane; k < bcnt; k += 32) {
+            const int t = (by0 + k / bw - v.row0) * v.gx + bx0 + k % bw;
+            const int64_t pos = (int64_t)tile_start[t] + atomicAdd(cursor + t * CSTRIDE, 1);
+            if (pos < capacity) { direct_key[pos] = bkey; direct_val[pos] = bid; }
+          }
+          continue;
+        }
+        for (int ry = 0; ry < bh; ry += 32) {
+          const int nr = min(32, bh - ry), r_lane = by0 + ry + lane - v.row0;
+          int rb = 0;
+          if (lane < nr) rb = tile_start[r_lane * v.gx] + atomicAdd(cursor + r_lane * v.gx * CSTRIDE + 2, bw);
+          for (int k0 = 0; k0 < nr * bw; k0 += 32) {
+            const int k = k0 + lane;
+            const int p = __shfl_sync(0xffffffffu, rb, k < nr * bw ? k / bw : 0);
+            if (k < nr * bw) {
+              const int64_t pos = (int64_t)p + k % bw;
+              if (pos < capacity) {
+                stage[pos] = composite(bkey, bid);
+                stage_tile[pos] = (by0 + ry + k / bw - v.row0) * v.gx + bx0 + k % bw;
+              }
+            }
+          }
+        }
+      }
+      // flush when the next round might not fit, and at the end of the chunk (everybody reads s_fill before anybody adds
+      // to it again: __syncthreads_or is the second barrier)
+      __syncthreads();
+      if (__syncthreads_or(s_fill > (round == rounds - 1 ? 0 : PART_FLUSH_AT))) flush();
+    }      // rounds
+  }      // chunks
+}
+
+// One chunk of PLACE_CHUNK staged instances per CTA and loop, chunks taken in staging order.  The chunk is counting-sorted
+// by tile in shared memory, so that consecutive lanes store consecutive slots of one tile's list (a warp's store touches
+// a few sectors instead of 32), and each tile's slots are reserved with one global atomic per chunk.
+__global__ void __launch_bounds__(BIN_THREADS)
+bin_place_kernel(int gx, int ntiles, const int32_t* __restrict__ tile_start, int32_t* __restrict__ cursor,
+                 const unsigned long long* __restrict__ stage, const int32_t* __restrict__ stage_tile, uint32_t* __restrict__ inst_key,
+                 uint32_t* __restrict__ inst_val) {
+  // bucket b < PLACE_WINDOW: tile t0 + b (t0 = the first tile of the chunk's first row); bucket PLACE_WINDOW: every tile
+  // beyond (a chunk spanning many sparse rows), placed straight from registers with one global atomic each
+  constexpr int PER = (PLACE_WINDOW + 1) / BIN_THREADS;      // buckets per thread in the scan
+  static_assert(PER * BIN_THREADS == PLACE_WINDOW + 1, "bucket count");
+  __shared__ int s_cnt[PLACE_WINDOW + 1];      // counts, then the chunk's offset of each bucket
+  __shared__ int s_base[PLACE_WINDOW];         // list position of the bucket's first entry, minus its chunk offset
+  __shared__ unsigned long long s_e[PLACE_CHUNK];
+  __shared__ uint16_t s_b[PLACE_CHUNK];
+  __shared__ int s_wsum[BIN_THREADS / 32];
+  __shared__ int s_t0;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int total = tile_start[ntiles];      // 0 after clamp_lists_kernel emptied the lists of an overflowing call
+  for (int beg = blockIdx.x * PLACE_CHUNK; beg < total; beg += gridDim.x * PLACE_CHUNK) {
+    for (int j = threadIdx.x; j <= PLACE_WINDOW; j += BIN_THREADS) s_cnt[j] = 0;
+    if (threadIdx.x == 0) s_t0 = stage_tile[beg] - stage_tile[beg] % gx;
+    __syncthreads();
+    const int t0 = s_t0;
+    int tk[PLACE_ITEMS], rank[PLACE_ITEMS];      // tile, then bucket; rank in the bucket
+#pragma unroll
+    for (int k = 0; k < PLACE_ITEMS; k++) {
+      const int idx = beg + k * BIN_THREADS + threadIdx.x;
+      tk[k] = idx < total ? stage_tile[idx] : -1;
     }
+#pragma unroll
+    for (int k = 0; k < PLACE_ITEMS; k++) {
+      rank[k] = 0;
+      if (tk[k] >= 0) {
+        const int b = min(tk[k] - t0, PLACE_WINDOW);
+        rank[k] = b < PLACE_WINDOW ? atomicAdd(&s_cnt[b], 1) : tile_start[tk[k]] + atomicAdd(cursor + tk[k] * CSTRIDE, 1);
+        tk[k] = b;      // from here on: the bucket (the outside bucket's rank is its list position)
+      }
+    }
+    __syncthreads();
+    // per thread PER consecutive buckets: reserve the tiles' slots, then a block-wide exclusive scan of the counts
+    int c[PER], sum = 0;
+    const int b0 = threadIdx.x * PER;
+    int32_t* const cur = cursor + (int64_t)(t0 + b0) * CSTRIDE;
+#pragma unroll
+    for (int q = 0; q < PER; q++) {
+      c[q] = s_cnt[b0 + q];
+      sum += c[q];
+    }
+#pragma unroll
+    for (int q = 0; q < PER; q++)
+      if (c[q] > 0 && b0 + q < PLACE_WINDOW) s_base[b0 + q] = tile_start[t0 + b0 + q] + atomicAdd(cur + q * CSTRIDE, c[q]);
+    int x = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) s_wsum[wid] = x;
+    __syncthreads();
+    int off = x - sum;
+#pragma unroll
+    for (int w = 0; w < BIN_THREADS / 32; w++) if (w < wid) off += s_wsum[w];
+#pragma unroll
+    for (int q = 0; q < PER; q++) {
+      const int b = threadIdx.x * PER + q;
+      s_cnt[b] = off;
+      if (b < PLACE_WINDOW && c[q] > 0) s_base[b] -= off;
+      off += c[q];
+    }
+    __syncthreads();
+    // the chunk in bucket order in shared memory (the outside bucket goes straight to its lists)
+#pragma unroll
+    for (int k = 0; k < PLACE_ITEMS; k++) {
+      if (tk[k] >= 0) {
+        const unsigned long long e = stage[beg + k * BIN_THREADS + threadIdx.x];
+        const int b = tk[k];
+        if (b < PLACE_WINDOW) {
+          const int j = s_cnt[b] + rank[k];
+          s_e[j] = e; s_b[j] = (uint16_t)b;
+        } else {
+          inst_key[rank[k]] = (uint32_t)(e >> 32); inst_val[rank[k]] = (uint32_t)e;
+        }
+      }
+    }
+    __syncthreads();
+    const int inside = s_cnt[PLACE_WINDOW];
+    for (int j = threadIdx.x; j < inside; j += BIN_THREADS) {      // consecutive j: consecutive slots of one list
+      const int pos = s_base[s_b[j]] + j;
+      const unsigned long long e = s_e[j];
+      inst_key[pos] = (uint32_t)(e >> 32); inst_val[pos] = (uint32_t)e;
+    }
+    __syncthreads();      // the shared arrays are reused by the next chunk
   }
-  }      // rows
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -283,8 +488,6 @@ struct MsdShared {
   int stack_beg[MSD_STACK], stack_len[MSD_STACK];
   int top, shift, overflow;
 };
-
-__device__ __forceinline__ unsigned long long composite(uint32_t k, uint32_t v) { return ((unsigned long long)k << 32) | v; }
 
 // Sorts (kA, vA)[0, len) in place; (kB, vB) is scratch of the same size.  Returns false if the work stack overflowed
 // (the caller then falls back to the LSD sort, which is always correct).
@@ -523,9 +726,10 @@ int launch_point_compact(int64_t n, const int32_t* count, int32_t* blk, int32_t*
   return 0;
 }
 
-int launch_tile_scan(int ntiles, int32_t* tile_start, int32_t* cursor, int32_t* meta, bool ranked, cudaStream_t st) {
+// `ranked` is ignored: the counting pass takes no slots (lgr_view.tile_rank_d is no longer read)
+int launch_tile_scan(int ntiles, int32_t* tile_start, int32_t* cursor, int32_t* meta, bool /* ranked */, cudaStream_t st) {
   ProfScope ps(K_TILE_SCAN, st);
-  tile_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(ntiles, tile_start, cursor, meta, SORT_CAP_SMALL_FWD, ranked ? 1 : 0);
+  tile_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(ntiles, tile_start, cursor, meta, SORT_CAP_SMALL_FWD);
   LGR_CHECK_LAUNCH();
   return 0;
 }
@@ -534,6 +738,8 @@ constexpr int LONG_SORT_GRID = 132;     // H100 SXM: 132 SMs. Device-sized long-
 
 // meta_dev != nullptr: device-sized call -- num_inst is the CAPACITY of the instance buffers, max_len / num_long are ignored
 // (read from meta_dev on the device), tile_start is mutable (emptied on overflow).
+// inst_tmp (2 x num_inst) is the staging buffer of the binning (and later the sort's scratch); sorted_ids holds the staged
+// tiles until the sort writes it.
 int launch_bin_and_sort(const View& v, int64_t n, int64_t num_inst, int max_len, int num_long, const float* splat,
                         const int32_t* radii, int32_t* tile_start, int32_t* cursor, uint32_t* inst_key,
                         uint32_t* inst_val, uint32_t* inst_tmp, int32_t* sorted_ids, int32_t* meta_dev, cudaStream_t st) {
@@ -543,19 +749,37 @@ int launch_bin_and_sort(const View& v, int64_t n, int64_t num_inst, int max_len,
     clamp_lists_kernel<<<(nt + 256) / 256, 256, 0, st>>>(nt, num_inst, tile_start, meta_dev);
     LGR_CHECK_LAUNCH();
   }
-  // With no binned instance only the sort is skipped: in band mode the scatter kernel is also the one writer of the
+  // With no binned instance only the sort is skipped: in band mode bin_partition is also the one writer of the
   // row -> id map and of the zeroed accumulator rows the backward reads (band lists follow the stock rectangle, so they
   // can be non-empty while nothing reaches alpha >= 1/255), and with band_dsplat set it zeroes the visible rows.
   if (num_inst == 0 && v.num_owners == 0 && v.band_dsplat == nullptr) return 0;
+  if (num_inst > 0 && (!inst_tmp || !sorted_ids)) return LGR_E_BADARG;
   const int ntiles = v.gx * (v.row1 - v.row0);
-  unsigned blocks = (unsigned)((n + SCATTER_THREADS - 1) / SCATTER_THREADS);
-  if (v.region_count && blocks > (unsigned)LGR_REGION_GRID) blocks = (unsigned)LGR_REGION_GRID;      // strides over the used rows (count known on the device only)
+  const int part_smem = part_smem_bytes(v.row1 - v.row0);
+  if (part_smem > 160 * 1024) return LGR_E_UNSUPPORTED;      // more than 13653 tile rows (218448 pixels) in one call
   {
-    ProfScope ps(K_BIN_SCATTER, st);
-    bin_scatter_kernel<<<blocks, SCATTER_THREADS, 0, st>>>(v, n, splat, radii, tile_start, cursor, inst_key, inst_val,
-                                                           meta_dev ? num_inst : (int64_t)0x7fffffffffffffffLL);
+    cudaError_t e = cudaFuncSetAttribute(bin_partition_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, part_smem);
+    if (e != cudaSuccess) return (int)e;
   }
-  LGR_CHECK_LAUNCH();
+  // a chunk of up to PART_ROUNDS x 256 Gaussians per CTA, fewer for small inputs so that the grid still fills the GPU
+  const int rounds = (int)max((int64_t)1, min((int64_t)PART_ROUNDS, n / ((int64_t)BIN_THREADS * 132 * 16)));
+  const int64_t chunk = (int64_t)rounds * BIN_THREADS;
+  unsigned blocks = (unsigned)((n + chunk - 1) / chunk);
+  if (v.region_count && blocks > (unsigned)LGR_REGION_GRID) blocks = (unsigned)LGR_REGION_GRID;      // strides over the used rows (count known on the device only)
+  unsigned long long* stage = reinterpret_cast<unsigned long long*>(inst_tmp);
+  {
+    ProfScope ps(K_BIN_SCATTER, st, num_inst > BIN_DIRECT_MAX ? 2 : 1);
+    // small views (lists well inside L2, where the scattered stores cost nothing extra): one kernel, no staging
+    const bool direct = num_inst <= BIN_DIRECT_MAX;
+    bin_partition_kernel<<<blocks, BIN_THREADS, part_smem, st>>>(v, n, splat, radii, tile_start, cursor, stage, sorted_ids, num_inst,
+                                                                 rounds, direct ? inst_key : nullptr, direct ? inst_val : nullptr);
+    LGR_CHECK_LAUNCH();
+    if (num_inst > 0 && !direct) {      // host-sized: num_inst = the instances; device-sized: the capacity (the count is read on the device)
+      const unsigned place = (unsigned)min((int64_t)PLACE_GRID, (num_inst + PLACE_CHUNK - 1) / PLACE_CHUNK);
+      bin_place_kernel<<<place, BIN_THREADS, 0, st>>>(v.gx, ntiles, tile_start, cursor, stage, sorted_ids, inst_key, inst_val);
+      LGR_CHECK_LAUNCH();
+    }
+  }
   if (num_inst == 0) return 0;
   int id_bits = 8;
   while (id_bits < 32 && (n - 1) >> id_bits) id_bits += 8;
@@ -584,7 +808,6 @@ int launch_bin_and_sort(const View& v, int64_t n, int64_t num_inst, int max_len,
     tile_sort_kernel<0><<<num_long, SORT_THREADS, 16 * cap, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_SMALL, cap, id_bits, nullptr, nullptr);
     LGR_CHECK_LAUNCH();
     if (max_len > SORT_CAP_LARGE) {
-      if (!inst_tmp) return LGR_E_CAPACITY;
       tile_sort_kernel<1><<<num_long, SORT_THREADS, 0, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_LARGE, 0, id_bits, nullptr, nullptr);
       LGR_CHECK_LAUNCH();
     }

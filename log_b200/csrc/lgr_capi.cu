@@ -153,7 +153,7 @@ int lgr_forward_project(const lgr_view* view, int64_t n, const float* means3D_d,
   if (rc) return rc;
   rc = launch_band_scan(v, st);
   if (rc) return rc;
-  return launch_tile_scan(ntiles, tile_start_d, tile_cursor_d, meta_d, view->tile_rank_d != nullptr, st);
+  return launch_tile_scan(ntiles, tile_start_d, tile_cursor_d, meta_d, false, st);
 }
 
 int lgr_forward_render(const lgr_view* view, int64_t n, int64_t num_instances, int32_t max_tile_len,
@@ -165,7 +165,7 @@ int lgr_forward_render(const lgr_view* view, int64_t n, int64_t num_instances, i
   if (!view_ok(view) || n < 0 || num_instances < 0 || num_long_tiles < 0 || !tile_start_d || !tile_cursor_d || !image_d || !final_T_d ||
       !n_contrib_d)
     return LGR_E_BADARG;
-  if (num_instances > 0 && (!inst_key_d || !inst_val_d || !sorted_ids_d || !splat_d || !radii_d)) return LGR_E_BADARG;
+  if (num_instances > 0 && (!inst_key_d || !inst_val_d || !inst_tmp_d || !sorted_ids_d || !splat_d || !radii_d)) return LGR_E_BADARG;
   if (const int rc6 = six_channels_check(view)) return rc6;
   if (view->want_aux && (!point_id_pixel_d || !point_weight_pixel_d || (n > 0 && !point_weight_d))) return LGR_E_BADARG;
   if (num_instances > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
@@ -182,11 +182,11 @@ int lgr_forward_render(const lgr_view* view, int64_t n, int64_t num_instances, i
 int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t instance_capacity, int32_t* meta_d,
                                     const float* splat_d, const int32_t* radii_d, int32_t* tile_start_d,
                                     int32_t* tile_cursor_d, uint32_t* inst_key_d, uint32_t* inst_val_d,
-                                    int32_t* sorted_ids_d, float* image_d, float* final_T_d, int32_t* n_contrib_d,
+                                    uint32_t* inst_tmp_d, int32_t* sorted_ids_d, float* image_d, float* final_T_d, int32_t* n_contrib_d,
                                     int32_t* point_id_pixel_d, float* point_weight_pixel_d, float* point_weight_d,
                                     int32_t* point_count_d, void* stream) {
   if (!view_ok(view) || n < 0 || instance_capacity <= 0 || !meta_d || !tile_start_d || !tile_cursor_d || !image_d || !final_T_d ||
-      !n_contrib_d || !inst_key_d || !inst_val_d || !sorted_ids_d)
+      !n_contrib_d || !inst_key_d || !inst_val_d || !inst_tmp_d || !sorted_ids_d)
     return LGR_E_BADARG;
   if (n > 0 && (!splat_d || !radii_d)) return LGR_E_BADARG;
   if (const int rc6 = six_channels_check(view)) return rc6;
@@ -197,7 +197,7 @@ int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t ins
   cudaStream_t st = (cudaStream_t)stream;
   const View v = make_view(view, n);
   int rc = launch_bin_and_sort(v, n, instance_capacity, 0, 0, splat_d, radii_d, tile_start_d, tile_cursor_d, inst_key_d, inst_val_d,
-                               nullptr, sorted_ids_d, meta_d, st);
+                               inst_tmp_d, sorted_ids_d, meta_d, st);
   if (rc) return rc;
   return launch_blend_fwd(v, tile_start_d, sorted_ids_d, splat_d, image_d, final_T_d, n_contrib_d, point_id_pixel_d,
                           point_weight_pixel_d, point_weight_d, view->want_aux ? point_count_d : nullptr, st);
@@ -441,7 +441,7 @@ int lgr_shard_recv_bin_aux(const lgr_view* view, const lgr_shard_layout* layout,
   int rc = launch_shard_recv_count(v, make_layout(layout), exchange_d, dsplat_d, tile_cursor_d, meta_d, point_weight_rows_d,
                                    point_count_rows_d, st);
   if (rc) return rc;
-  return launch_tile_scan(ntiles, tile_start_d, tile_cursor_d, meta_d, view->tile_rank_d != nullptr, st);
+  return launch_tile_scan(ntiles, tile_start_d, tile_cursor_d, meta_d, false, st);
 }
 
 int lgr_blend_backward(const lgr_view* view, int64_t n, int64_t num_instances, const float* splat_d,

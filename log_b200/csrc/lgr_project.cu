@@ -257,7 +257,7 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
         if (DEPTH) r3 = make_float4(cv.t[2], p[2], 1.0f, 0.f);
         if (reach) {
           tile_rect_tight(px, py, rad, hx, hy, v.gx, v.gy, v.row0, v.row1, x0, y0, x1, y1);
-          big_splat = count_small_tiles(v, tile_count, i, x0, y0, x1, y1);
+          big_splat = count_small_tiles(v, tile_count, x0, y0, x1, y1);
           bx0 = x0; by0 = y0; bx1 = x1; by1 = y1;
         }
       }

@@ -198,7 +198,7 @@ shard_recv_count_kernel(View v, ShardLayout L, float* __restrict__ xbuf, float* 
       stock += (unsigned)((x1 - x0) * max(0, min(y1, v.row1) - max(y0, v.row0)));
       vis += 1;
       tile_rect_tight(r0.x, r0.y, rad, r1.z, r1.w, v.gx, v.gy, v.row0, v.row1, x0, y0, x1, y1);
-      big_splat = count_small_tiles(v, tile_count, slot, x0, y0, x1, y1);
+      big_splat = count_small_tiles(v, tile_count, x0, y0, x1, y1);
       bx0 = x0; by0 = y0; bx1 = x1; by1 = y1;
       float4* z = reinterpret_cast<float4*>(dsplat + slot * LGR_GRAD_FLOATS);
       z[0] = z[1] = z[2] = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -27,8 +27,6 @@ from . import _capi
 from ._capi import LGR_FILTER_ADD, LGR_FILTER_MAX, LGR_FILTER_NONE, LgrView
 
 PREZERO_DSPLAT = bool(int(__import__('os').environ.get('LGR_PREZERO_DSPLAT', '0')))      # see rasterize_forward
-# tile slots taken once, by the counting pass (lgr_view.tile_rank_d); 0 = the two-pass binning of round 1 (A/B knob)
-RANKED_BIN = bool(int(__import__('os').environ.get('LGR_RANKED_BIN', '1')))
 # the forward blend lists the entries some pixel composited, with their sub-tiles; the backward stages and walks only those (A/B knob)
 CONTRIB_BITS = bool(int(__import__('os').environ.get('LGR_CONTRIB_BITS', '1')))
 FLAVOUR_STOCK = 'stock'   # diff_gaussian_rasterization            (graphdeco-inria)   -> 2-tuple, cov += 0.3
@@ -77,7 +75,7 @@ def _stream(device=None):
 
 def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: bool, sh_coeffs: int, tile_rows, keep,
                num_owners=0, band_ids=None, band_count=None, band_blk=None, band_rows=None, band_dsplat=None,
-               raw_params=False, tile_rank=None, gather_index=None, pid_map=None, cov3D_precomp=None, splat_ext=None,
+               raw_params=False, gather_index=None, pid_map=None, cov3D_precomp=None, splat_ext=None,
                log_depth=False):
     dev = s.viewmatrix.device
     vm, pm = _f32c(s.viewmatrix, 'viewmatrix'), _f32c(s.projmatrix, 'projmatrix', dev)
@@ -98,7 +96,6 @@ def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: boo
     v.band_blk_d = band_blk.data_ptr() if band_blk is not None else None
     v.band_rows_d = band_rows.data_ptr() if band_rows is not None else None
     v.band_dsplat_d = band_dsplat.data_ptr() if band_dsplat is not None else None
-    v.tile_rank_d = tile_rank.data_ptr() if tile_rank is not None else None
     v.gather_index_d = gather_index.data_ptr() if gather_index is not None else None
     v.pid_map_d = pid_map.data_ptr() if pid_map is not None else None
     v.cov3D_precomp_d = cov3D_precomp.data_ptr() if cov3D_precomp is not None else None
@@ -230,7 +227,7 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     if prezero_dsplat is None:
         prezero_dsplat = PREZERO_DSPLAT and torch.is_grad_enabled()
     if num_owners == 0 and prezero_dsplat:
-        # experiment (LGR_PREZERO_DSPLAT=1): the scatter kernel zeroes the accumulator rows the backward will read, instead of a
+        # experiment (LGR_PREZERO_DSPLAT=1): the binning kernel zeroes the accumulator rows the backward will read, instead of a
         # 48 N-byte memset at the start of the backward
         band_dsplat = torch.empty((max(n, 1), _capi.LGR_GRAD_FLOATS), dtype=torch.float32, device=dev)
     if num_owners > 0:
@@ -240,12 +237,10 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         band_ids = torch.empty((max(256 * nb, 1),), dtype=torch.int32, device=dev)
         band_blk = torch.empty((2 * nb + 1,), dtype=torch.int32, device=dev)
         band_count = torch.empty((num_owners,), dtype=torch.int32, device=dev)
-    tile_rank = torch.empty((max(n, 1), 4), dtype=torch.int32, device=dev) if RANKED_BIN else None
-    keep.append(tile_rank)
     splat_ext = torch.empty((max(n, 1), 4), dtype=torch.float32, device=dev) if channels == 6 else None      # never NULL
     keep.append(splat_ext)
     view = _make_view(settings, filter_mode, want_aux, K, tile_rows, keep, num_owners, band_ids, band_count, band_blk, band_rows, band_dsplat,
-                      raw_params, tile_rank, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext, log_depth=log_depth)
+                      raw_params, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext, log_depth=log_depth)
     H, W = view.image_height, view.image_width
     gx, gy = (W + 15) // 16, (H + 15) // 16
     rows = gy if tile_rows is None else int(tile_rows[1]) - int(tile_rows[0])
@@ -279,12 +274,13 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
             raise _capi.LgrError('instance_capacity (device-sized call) is not available in band mode')
         D, max_len, num_long, stock_D, m = int(instance_capacity), None, None, None, None
         inst_key, inst_val = torch.empty((D,), **u32), torch.empty((D,), **u32)
+        inst_tmp = torch.empty((2 * D,), **u32)      # the binning's staging buffer
         sorted_ids = torch.empty((D,), **i32)
         contrib = torch.empty((2 * D + ntiles,), **i32) if use_contrib_lists(D, None) else None
         keep.append(contrib)
         set_contrib_lists(view, contrib, D, n_contrib)
         _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(view), n, D, _ptr(meta), _ptr(splat), _ptr(radii), _ptr(tile_start),
-                                                        _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(sorted_ids), _ptr(image),
+                                                        _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp), _ptr(sorted_ids), _ptr(image),
                                                         _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp), _ptr(pw), _ptr(pc), st),
                     'lgr_forward_render_device_sized')
     else:
@@ -296,7 +292,7 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
                                  f'{m[4]} of {n} Gaussians visible, longest tile list {max_len}): more than 2^31 - 1 is unsupported')
         inst_key = torch.empty((D,), **u32)
         inst_val = torch.empty((D,), **u32)
-        inst_tmp = torch.empty((2 * D,), **u32) if max_len > lib.lgr_sort_smem_capacity() else None
+        inst_tmp = torch.empty((2 * D,), **u32)      # the binning's staging buffer, then the sort's scratch for lists beyond shared memory
         sorted_ids = torch.empty((D,), **i32)
         # forward -> backward: the entries some pixel composited (lgr_view.contrib_*); the backward stages only those and
         # stops a pixel after its last contributor
@@ -332,7 +328,7 @@ def rasterize_backward(state: RasterState, grad_image, means3D, opacities, scale
     f32 = dict(dtype=torch.float32, device=dev)
     g = _f32c(grad_image, 'grad_image', dev)
     if state.band_ids[3] is not None:
-        dsplat = state.band_ids[3]          # rows the backward reads were zeroed by the forward's scatter kernel
+        dsplat = state.band_ids[3]          # rows the backward reads were zeroed by the forward's binning kernel
         state.band_ids = state.band_ids[:3] + (None,)      # one backward per forward
     else:
         dsplat = torch.zeros((n, _capi.LGR_GRAD_FLOATS), **f32)

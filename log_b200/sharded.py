@@ -290,9 +290,7 @@ class SplatExchange:
         s.keep, s.n, s.want_aux, s.settings = [], n, bool(want_aux), settings
         K = 0 if sh is None else int(sh.shape[1])
         s.view_full = _make_view(settings, filter_mode, want_aux, K, None, s.keep, raw_params=raw_params)
-        from .rasterizer import RANKED_BIN
-        rank_rows = self._scratch('tile_rank', (self.world * self.cap, 4), torch.int32) if RANKED_BIN else None
-        s.view_band = _make_view(settings, filter_mode, want_aux, K, self.band, s.keep, raw_params=raw_params, tile_rank=rank_rows,
+        s.view_band = _make_view(settings, filter_mode, want_aux, K, self.band, s.keep, raw_params=raw_params,
                                  pid_map=self.recv_gid)      # point_id_pixel: received row -> global Gaussian index, in the kernel
         # the receive and render kernels visit only the rows the sources filled (the first count[s] of each region)
         s.view_band.region_count_d = self.buf.data_ptr() + 4 * int(self.layout.off_count)
@@ -354,12 +352,13 @@ class SplatExchange:
             cap = self._inst_cap
             inst_key = self._scratch('inst_key', (cap,), torch.int32)
             inst_val = self._scratch('inst_val', (cap,), torch.int32)
+            inst_tmp = self._scratch('inst_tmp', (2 * cap,), torch.int32)      # the binning's staging buffer
             s.sorted_ids = self._scratch('sorted_ids', (cap,), torch.int32)
             set_contrib_lists(v, self._scratch('contrib', (2 * cap + ntiles,), torch.int32) if use_contrib_lists(cap, None) else None,
                               cap, n_contrib)
             s.num_instances, s.max_tile_len, s.num_rows, s.stock_instances = cap, None, None, None      # see stats()
             _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(v), rows, cap, _ptr(meta), _ptr(self.recv_splat), _ptr(self.recv_radii),
-                                                            _ptr(s.tile_start), _ptr(cursor), _ptr(inst_key), _ptr(inst_val), _ptr(s.sorted_ids),
+                                                            _ptr(s.tile_start), _ptr(cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp), _ptr(s.sorted_ids),
                                                             _ptr(s.image), _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp),
                                                             _ptr(s.pw_rows), _ptr(s.pc_rows), st), 'lgr_forward_render_device_sized')
             return s.image, s.radii, pid, pwp
@@ -372,7 +371,7 @@ class SplatExchange:
             self._inst_cap = max(self._inst_cap, D + D // 4 + 4096)
         inst_key = self._scratch('inst_key', (D,), torch.int32)
         inst_val = self._scratch('inst_val', (D,), torch.int32)
-        inst_tmp = self._scratch('inst_tmp', (2 * D,), torch.int32) if max_len > lib.lgr_sort_smem_capacity() else None
+        inst_tmp = self._scratch('inst_tmp', (2 * D,), torch.int32)      # the binning's staging buffer (and the sort's scratch)
         s.sorted_ids = self._scratch('sorted_ids', (D,), torch.int32)
         set_contrib_lists(v, self._scratch('contrib', (2 * D + ntiles,), torch.int32) if use_contrib_lists(D, max_len) else None,
                           D, n_contrib)
