@@ -197,11 +197,12 @@ int32_t lgr_sort_smem_capacity(void);
  * independent of D / the longest list / the number of long tiles -- the kernels read them from meta_d on the device -- so the
  * whole forward needs no host synchronisation and can be captured in a CUDA graph.  The caller sizes inst_key_d /
  * inst_val_d / sorted_ids_d for `instance_capacity` instances (e.g. 1.25 x the D of the previous view), inst_tmp_d for
- * 2 x instance_capacity (the binning's staging buffer, 8-byte aligned).  If the view needs
- * more (meta_d[0] > instance_capacity) or holds a tile list longer than lgr_sort_smem_capacity(), nothing is written out of
- * bounds, meta_d[6] is set to a non-zero value (bit 0: capacity, bit 1: list too long) and the outputs of this view are
- * INVALID: the caller checks meta_d[6] when it next synchronises and redoes the view through lgr_forward_render.
- * tile_start_d is mutable here (emptied on overflow). */
+ * 2 x instance_capacity (the binning's staging buffer, 8-byte aligned, and the sort's scratch for lists longer than
+ * lgr_sort_smem_capacity()).  Within its capacity the call bins and sorts exactly what lgr_forward_render does.  If the view
+ * needs more (meta_d[0] > instance_capacity) or holds a tile list longer than LGR_CONTRIB_MAX_LIST, every tile list is
+ * emptied, so nothing is read or written out of bounds, meta_d[6] is set to a non-zero value (bit 0: capacity, bit 1: list
+ * too long) and the outputs of this view are INVALID: the caller checks meta_d[6] when it next synchronises and redoes the
+ * view through lgr_forward_render.  tile_start_d is mutable here (emptied on overflow). */
 int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t instance_capacity, int32_t* meta_d,
                                     const float* splat_d, const int32_t* radii_d, int32_t* tile_start_d,
                                     int32_t* tile_cursor_d, uint32_t* inst_key_d, uint32_t* inst_val_d,

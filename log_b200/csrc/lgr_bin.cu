@@ -587,31 +587,31 @@ __device__ __forceinline__ bool sort_tile_msd(uint32_t* kA, uint32_t* vA, uint32
   return ok;
 }
 
-// mode 0: lists with len <= cap live in shared memory (dynamic smem = 16*cap bytes); longer lists are skipped.
-// mode 1: lists with lo < len are sorted in global memory (inst_* in place, tmp_* scratch).
+// MODE 0: lists with lo < len <= cap are sorted in shared memory (dynamic smem = 16*cap bytes); longer lists are left to a
+//         later launch.
+// MODE 1: lists with lo < len are sorted in global memory (inst_* in place, tmp_* scratch).
+// MODE 2: lists with lo < len, each where it fits: in shared memory up to cap, in global memory beyond (the device-sized
+//         long-tile launch, which cannot size a later launch by the longest list; the LSD histogram aliases the dynamic
+//         shared memory that the global path leaves unused).
 // count_ptr == nullptr: one tile per CTA (tile = tile_list ? tile_list[blockIdx.x] : blockIdx.x).  Otherwise the grid is a
 // fixed size and strides over the *count_ptr listed tiles (device-sized launch: no host read of the long-tile count).
-// flags (may be nullptr): bit 1 is set when a list longer than `cap` is met in MODE 0 with lo > 0 (a long-tile launch that
-// cannot hold it: the list stays unsorted and the caller must redo the step with the host-sized path).
 template <int MODE>
 __global__ void __launch_bounds__(SORT_THREADS)
 tile_sort_kernel(const int32_t* __restrict__ tile_list /* nullptr: tile = blockIdx.x */,
                  const int32_t* __restrict__ tile_start, uint32_t* __restrict__ inst_key,
                  uint32_t* __restrict__ inst_val, uint32_t* __restrict__ tmp, int32_t* __restrict__ sorted_ids, int lo,
-                 int cap, int id_bits, const int32_t* __restrict__ count_ptr, int32_t* __restrict__ flags) {
+                 int cap, int id_bits, const int32_t* __restrict__ count_ptr) {
   extern __shared__ uint32_t smem_u32[];
-  __shared__ int whist[MODE == 1 ? SORT_WARPS * RADIX : 1];
+  __shared__ int whist_s[MODE == 1 ? SORT_WARPS * RADIX : 1];
+  int* const whist = MODE == 2 ? reinterpret_cast<int*>(smem_u32) : whist_s;
   __shared__ MsdShared msd;
   const int count = count_ptr ? *count_ptr : (int)gridDim.x;
   for (int b = blockIdx.x; b < count; b += gridDim.x) {
     const int t = tile_list ? tile_list[b] : b;
     const int beg = tile_start[t], len = tile_start[t + 1] - beg;
     if (len <= lo) continue;
-    if (MODE == 0 && len > cap) {
-      if (flags && lo > 0 && threadIdx.x == 0) atomicOr(flags, 2);
-      continue;
-    }
-    if (MODE == 0) {
+    if (MODE == 0 && len > cap) continue;
+    if (MODE != 1 && len <= cap) {
       uint32_t* kA = smem_u32; uint32_t* vA = kA + cap; uint32_t* kB = vA + cap; uint32_t* vB = kB + cap;
       for (int i = threadIdx.x; i < len; i += SORT_THREADS) { kA[i] = inst_key[beg + i]; vA[i] = inst_val[beg + i]; }
       __syncthreads();
@@ -635,13 +635,15 @@ tile_sort_kernel(const int32_t* __restrict__ tile_list /* nullptr: tile = blockI
   }
 }
 
-// Device-sized binning (no host read of D): if more instances were counted than the caller's buffers hold, flag it (bit 0)
-// and empty every tile list, so that no later kernel reads or writes past `capacity`; the caller redoes the step.
+// Device-sized binning (no host read of D): if more instances were counted than the caller's buffers hold (bit 0), or a tile
+// list is longer than LGR_CONTRIB_MAX_LIST (bit 1: its entry indices would not fit lgr_view.contrib_entry_d), flag it and
+// empty every tile list, so that no later kernel reads or writes past `capacity`; the caller redoes the step.
 __global__ void __launch_bounds__(256)
 clamp_lists_kernel(int ntiles, int64_t capacity, int32_t* __restrict__ tile_start, int32_t* __restrict__ meta) {
-  if ((int64_t)meta[0] <= capacity) return;
+  const int flags = ((int64_t)meta[0] > capacity ? 1 : 0) | (meta[1] > LGR_CONTRIB_MAX_LIST ? 2 : 0);
+  if (!flags) return;
   for (int i = blockIdx.x * 256 + threadIdx.x; i <= ntiles; i += gridDim.x * 256) tile_start[i] = 0;
-  if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(meta + 6, 1);
+  if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(meta + 6, flags);
 }
 
 
@@ -785,30 +787,32 @@ int launch_bin_and_sort(const View& v, int64_t n, int64_t num_inst, int max_len,
   while (id_bits < 32 && (n - 1) >> id_bits) id_bits += 8;
   {      // per device / context and cheap: set on every call (a process may drive several GPUs)
     cudaError_t e = cudaFuncSetAttribute(tile_sort_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * SORT_CAP_LARGE);
+    if (e == cudaSuccess && meta_dev) e = cudaFuncSetAttribute(tile_sort_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * SORT_CAP_LARGE);
     if (e != cudaSuccess) return (int)e;
   }
   if (meta_dev) {
     // device-sized: launch shapes do not depend on D / longest list / number of long tiles (read on the device), so the
     // forward needs no host synchronisation and can be captured in a CUDA graph
     ProfScope ps(K_TILE_SORT, st, 2);
-    tile_sort_kernel<0><<<ntiles, SORT_THREADS, 16 * SORT_CAP_SMALL, st>>>(nullptr, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, 0, SORT_CAP_SMALL, id_bits, nullptr, nullptr);
+    tile_sort_kernel<0><<<ntiles, SORT_THREADS, 16 * SORT_CAP_SMALL, st>>>(nullptr, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, 0, SORT_CAP_SMALL, id_bits, nullptr);
     LGR_CHECK_LAUNCH();
+    // every list longer than the main launch holds, however long: a device-sized call sorts what the host-sized one does
     const int32_t* long_list = cursor + CSTRIDE * ntiles;
-    tile_sort_kernel<0><<<LONG_SORT_GRID, SORT_THREADS, 16 * SORT_CAP_LARGE, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_SMALL, SORT_CAP_LARGE, id_bits, meta_dev + 5, meta_dev + 6);
+    tile_sort_kernel<2><<<LONG_SORT_GRID, SORT_THREADS, 16 * SORT_CAP_LARGE, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_SMALL, SORT_CAP_LARGE, id_bits, meta_dev + 5);
     LGR_CHECK_LAUNCH();
     return 0;
   }
   ProfScope ps(K_TILE_SORT, st, 1 + (num_long > 0) + (max_len > SORT_CAP_LARGE));
   const int cap_main = max(256, min(max_len, SORT_CAP_SMALL));
-  tile_sort_kernel<0><<<ntiles, SORT_THREADS, 16 * cap_main, st>>>(nullptr, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, 0, cap_main, id_bits, nullptr, nullptr);
+  tile_sort_kernel<0><<<ntiles, SORT_THREADS, 16 * cap_main, st>>>(nullptr, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, 0, cap_main, id_bits, nullptr);
   LGR_CHECK_LAUNCH();
   if (num_long > 0) {   // only the long tiles (listed by the scan kernel behind the cursors), smem sized to the longest
     const int32_t* long_list = cursor + CSTRIDE * ntiles;
     const int cap = min(max_len, SORT_CAP_LARGE);
-    tile_sort_kernel<0><<<num_long, SORT_THREADS, 16 * cap, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_SMALL, cap, id_bits, nullptr, nullptr);
+    tile_sort_kernel<0><<<num_long, SORT_THREADS, 16 * cap, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_SMALL, cap, id_bits, nullptr);
     LGR_CHECK_LAUNCH();
     if (max_len > SORT_CAP_LARGE) {
-      tile_sort_kernel<1><<<num_long, SORT_THREADS, 0, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_LARGE, 0, id_bits, nullptr, nullptr);
+      tile_sort_kernel<1><<<num_long, SORT_THREADS, 0, st>>>(long_list, tile_start, inst_key, inst_val, inst_tmp, sorted_ids, SORT_CAP_LARGE, 0, id_bits, nullptr);
       LGR_CHECK_LAUNCH();
     }
   }

@@ -192,8 +192,8 @@ int lgr_forward_render_device_sized(const lgr_view* view, int64_t n, int64_t ins
   if (const int rc6 = six_channels_check(view)) return rc6;
   if (view->want_aux && (!point_id_pixel_d || !point_weight_pixel_d || (n > 0 && !point_weight_d))) return LGR_E_BADARG;
   if (instance_capacity > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
-  // contrib_entry_d's list indices: a list longer than lgr_sort_smem_capacity() (far below LGR_CONTRIB_MAX_LIST) already
-  // raises meta_d[6] bit 1, so no valid output of this call depends on an index that did not fit
+  // contrib_entry_d's list indices: a list longer than LGR_CONTRIB_MAX_LIST raises meta_d[6] bit 1 and empties every list,
+  // so no valid output of this call depends on an index that did not fit
   cudaStream_t st = (cudaStream_t)stream;
   const View v = make_view(view, n);
   int rc = launch_bin_and_sort(v, n, instance_capacity, 0, 0, splat_d, radii_d, tile_start_d, tile_cursor_d, inst_key_d, inst_val_d,

@@ -151,7 +151,7 @@ def colour_channels(colors_precomp, settings, shs=None, raw_params=False, gather
 
 def use_contrib_lists(D, max_tile_len):
     """Record the contribution lists for the backward?  (Not for an empty view, nor for a tile list longer than the entry
-    word's index field; max_tile_len None: a device-sized call, whose lists are bounded by lgr_sort_smem_capacity().)"""
+    word's index field; max_tile_len None: a device-sized call, which empties its lists and flags the view when one is longer.)"""
     return CONTRIB_BITS and D > 0 and (max_tile_len is None or max_tile_len <= _capi.LGR_CONTRIB_MAX_LIST)
 
 
@@ -164,7 +164,8 @@ class RasterState:
 
     def read_stats(self):
         """Counters of this forward, read back from meta_d (synchronises): D, longest tile list, D by the stock rule, visible
-        Gaussians, and `overflow` (non-zero only after a device-sized call that outgrew its buffers: outputs invalid)."""
+        Gaussians, and `overflow` (non-zero only after a device-sized call whose view outgrew its buffers, bit 0, or held a
+        tile list longer than LGR_CONTRIB_MAX_LIST entries, bit 1: outputs invalid, redo the view host-sized)."""
         m = self.meta.tolist()
         return dict(num_instances=int(m[0]), max_tile_len=int(m[1]), stock_instances=(m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32),
                     num_visible=int(m[4]), overflow=int(m[6]))
