@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 24
+#define LGR_ABI_VERSION 25
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -501,6 +501,44 @@ int lgr_ssim_forward(int32_t batch, int32_t channels, int32_t height, int32_t wi
 int lgr_ssim_backward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* img1_d,
                       const int64_t* strides1, const float* img2_d, const int64_t* strides2, const float* maps_d,
                       const float* grad_loss_d, float* grad_img1_d, void* stream);
+
+/* LoG's photometric loss (NaiveRendererAndLoss.calculate_loss, renderer.py:253-266) in the same three kernels:
+ *     x   = gt m + render (1 - m)  per pixel when mask_d is given (m = mask_ignore), else the render
+ *     ssim = 1 - mean(S) of (x, gt) as lgr_ssim_forward,   l1 = mean |r1 - gt| over B C H W,
+ *     loss = fl(fl(0.2 ssim) + fl(0.8 l1)),
+ * r1 = render_l1_d (LoG's render_correct[:, :3], read unblended) or, when NULL, x itself.  Written to loss_d, l1_d and
+ * ssim_d, one float each, on the device.
+ *   render_d, gt_d, render_l1_d: fp32 (B, C, H, W) read through the element strides (HOST arrays of 4 int64)
+ *   mask_d:         NULL or fp32 (B, H, W), strides mask_strides (HOST array of 3 int64)
+ *   scratch_d:      LGR_PHOTO_SCRATCH_DOUBLES(B, C, H, W) doubles: per-CTA SSIM and L1 partial sums, summed in a fixed
+ *                   order (the outputs repeat bit for bit)
+ *   maps_d:         NULL, or LGR_PHOTO_MAP_FLOATS(B, C, H, W) floats for lgr_photometric_backward */
+#define LGR_PHOTO_SCRATCH_DOUBLES(b, c, h, w) (2 * LGR_SSIM_SCRATCH_DOUBLES(b, c, h, w))
+#define LGR_PHOTO_MAP_FLOATS(b, c, h, w) LGR_SSIM_MAP_FLOATS(b, c, h, w)
+int lgr_photometric_forward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* render_d,
+                            const int64_t* render_strides, const float* gt_d, const int64_t* gt_strides, const float* mask_d,
+                            const int64_t* mask_strides, const float* render_l1_d, const int64_t* l1_strides,
+                            double* scratch_d, float* loss_d, float* l1_d, float* ssim_d, float* maps_d, void* stream);
+/* Its gradient, from three upstream scalars on the device (grad_loss_d, grad_l1_d, grad_ssim_d: dL/dloss, dL/dl1,
+ * dL/dssim): with gs = fl(0.2 grad_loss) + grad_ssim and gl = (fl(0.8 grad_loss) + grad_l1) / (B C H W),
+ *     grad_render_d    = (SSIM gradient for gs [+ sign(x - gt) gl when render_l1_d is NULL]) (1 - m)
+ *     grad_render_l1_d = sign(r1 - gt) gl   (only with render_l1_d; sign(0) = 0)
+ * both contiguous fp32 (B, C, H, W).  maps_d from the forward; the other arguments as in the forward. */
+int lgr_photometric_backward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* render_d,
+                             const int64_t* render_strides, const float* gt_d, const int64_t* gt_strides,
+                             const float* mask_d, const int64_t* mask_strides, const float* render_l1_d,
+                             const int64_t* l1_strides, const float* maps_d, const float* grad_loss_d,
+                             const float* grad_l1_d, const float* grad_ssim_d, float* grad_render_d,
+                             float* grad_render_l1_d, void* stream);
+
+/* LoG's Corrector.step (LoG/model/corrector.py:35-62) for view `index` of a (num_views, 3) view-correction table, one
+ * launch of one warp, no host read: steps_d[index] += 1; s = steps_d[index] - start_step; if s >= 0, AMSGrad Adam on
+ * row `index` with lr = exp(log_lr_init (1 - t) + log_lr_final t), t = clip(s / 100, 0, 1) in fp64, and LoG's float32
+ * tensor bias corrections 1 - 0.9^s, sqrt(1 - 0.999^s), eps 1e-15; then grad_d[index] = 0.  All tables contiguous on the
+ * device: steps_d int32 (num_views), the others fp32 (num_views, 3); max_exp_avg_sq_d may be NULL (no AMSGrad). */
+int lgr_corrector_step(int64_t num_views, int64_t index, int32_t start_step, double log_lr_init, double log_lr_final,
+                       int32_t* steps_d, float* param_d, float* grad_d, float* exp_avg_d, float* exp_avg_sq_d,
+                       float* max_exp_avg_sq_d, void* stream);
 
 /* Depth-supervision loss (LoG's NaiveRendererAndLoss.append_depth_loss, renderer.py:268-292, with MiDaS's
  * ScaleAndShiftInvariantLoss(alpha=0.5, scales=1), LoG/render/loss.py:47-117).  For each of the 64 patches k, the 64x64

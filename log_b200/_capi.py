@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 24
+LGR_ABI_VERSION = 25
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -22,7 +22,8 @@ EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'l
            'lgr_profile_kernel_name', 'lgr_shard_send', 'lgr_shard_recv_bin', 'lgr_blend_backward', 'lgr_shard_return_rows',
            'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible',
            'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis',
-           'lgr_counter_update', 'lgr_log_step', 'lgr_prepare_cull', 'lgr_prepare_select')
+           'lgr_counter_update', 'lgr_log_step', 'lgr_prepare_cull', 'lgr_prepare_select', 'lgr_photometric_forward',
+           'lgr_photometric_backward', 'lgr_corrector_step')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -80,6 +81,11 @@ LGR_SSIM_TILE = 32
 def ssim_scratch_doubles(b, c, h, w):
     """LGR_SSIM_SCRATCH_DOUBLES."""
     return b * c * ((h - LGR_SSIM_WINDOW + LGR_SSIM_TILE) // LGR_SSIM_TILE) * ((w - LGR_SSIM_WINDOW + LGR_SSIM_TILE) // LGR_SSIM_TILE)
+
+
+def photo_scratch_doubles(b, c, h, w):
+    """LGR_PHOTO_SCRATCH_DOUBLES."""
+    return 2 * ssim_scratch_doubles(b, c, h, w)
 
 
 def ssim_map_floats(b, c, h, w):
@@ -184,6 +190,12 @@ def bind(lib):
     lib.lgr_ssim_forward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     lib.lgr_ssim_backward.restype = ctypes.c_int
     lib.lgr_ssim_backward.argtypes = [_i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    lib.lgr_photometric_forward.restype = ctypes.c_int
+    lib.lgr_photometric_forward.argtypes = [_i32, _i32, _i32, _i32] + [_vp] * 14
+    lib.lgr_photometric_backward.restype = ctypes.c_int
+    lib.lgr_photometric_backward.argtypes = [_i32, _i32, _i32, _i32] + [_vp] * 15
+    lib.lgr_corrector_step.restype = ctypes.c_int
+    lib.lgr_corrector_step.argtypes = [_i64, _i64, _i32, ctypes.c_double, ctypes.c_double] + [_vp] * 7
     lib.lgr_depth_loss_forward.restype = ctypes.c_int
     lib.lgr_depth_loss_forward.argtypes = [_i32, _i32, _i32, _i32] + [_vp] * 11
     lib.lgr_depth_loss_backward.restype = ctypes.c_int

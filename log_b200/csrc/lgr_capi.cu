@@ -45,6 +45,13 @@ int launch_ssim_fwd(int, int, int, int, const float*, const int64_t*, const floa
                     cudaStream_t);
 int launch_ssim_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
                     const float*, float*, cudaStream_t);
+int launch_photometric_fwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
+                           const int64_t*, const float*, const int64_t*, double*, float*, float*, float*, float*,
+                           cudaStream_t);
+int launch_photometric_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
+                           const int64_t*, const float*, const int64_t*, const float*, const float*, const float*,
+                           const float*, float*, float*, cudaStream_t);
+int launch_corrector_step(int64_t, int32_t, double, double, int32_t*, float*, float*, float*, float*, float*, cudaStream_t);
 int launch_depth_loss_fwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
                           const int64_t*, const int64_t*, const int64_t*, double*, float*, cudaStream_t);
 int launch_depth_loss_bwd(int, int, int, int, const float*, const int64_t*, const float*, const int64_t*, const float*,
@@ -320,6 +327,58 @@ int lgr_ssim_backward(int32_t batch, int32_t channels, int32_t height, int32_t w
     return LGR_E_BADARG;
   return launch_ssim_bwd(batch, channels, height, width, img1_d, strides1, img2_d, strides2, maps_d, grad_loss_d,
                          grad_img1_d, (cudaStream_t)stream);
+}
+
+// What an lgr_photometric_* call adds to an lgr_ssim_* call: the optional mask and L1 image with their strides.
+static bool photo_args_ok(const float* mask_d, const int64_t* mask_strides, const float* render_l1_d,
+                          const int64_t* l1_strides) {
+  if (mask_d) {
+    if (!mask_strides) return false;
+    for (int k = 0; k < 3; k++)
+      if (mask_strides[k] < 0) return false;
+  }
+  if (render_l1_d) {
+    if (!l1_strides) return false;
+    for (int k = 0; k < 4; k++)
+      if (l1_strides[k] < 0) return false;
+  }
+  return true;
+}
+
+int lgr_photometric_forward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* render_d,
+                            const int64_t* render_strides, const float* gt_d, const int64_t* gt_strides, const float* mask_d,
+                            const int64_t* mask_strides, const float* render_l1_d, const int64_t* l1_strides,
+                            double* scratch_d, float* loss_d, float* l1_d, float* ssim_d, float* maps_d, void* stream) {
+  if (!ssim_args_ok(batch, channels, height, width, render_d, render_strides, gt_d, gt_strides) ||
+      !photo_args_ok(mask_d, mask_strides, render_l1_d, l1_strides) || !scratch_d || !loss_d || !l1_d || !ssim_d)
+    return LGR_E_BADARG;
+  return launch_photometric_fwd(batch, channels, height, width, render_d, render_strides, gt_d, gt_strides, mask_d,
+                                mask_strides, render_l1_d, l1_strides, scratch_d, loss_d, l1_d, ssim_d, maps_d,
+                                (cudaStream_t)stream);
+}
+
+int lgr_photometric_backward(int32_t batch, int32_t channels, int32_t height, int32_t width, const float* render_d,
+                             const int64_t* render_strides, const float* gt_d, const int64_t* gt_strides,
+                             const float* mask_d, const int64_t* mask_strides, const float* render_l1_d,
+                             const int64_t* l1_strides, const float* maps_d, const float* grad_loss_d,
+                             const float* grad_l1_d, const float* grad_ssim_d, float* grad_render_d,
+                             float* grad_render_l1_d, void* stream) {
+  if (!ssim_args_ok(batch, channels, height, width, render_d, render_strides, gt_d, gt_strides) ||
+      !photo_args_ok(mask_d, mask_strides, render_l1_d, l1_strides) || !maps_d || !grad_loss_d || !grad_l1_d ||
+      !grad_ssim_d || !grad_render_d || (render_l1_d && !grad_render_l1_d))
+    return LGR_E_BADARG;
+  return launch_photometric_bwd(batch, channels, height, width, render_d, render_strides, gt_d, gt_strides, mask_d,
+                                mask_strides, render_l1_d, l1_strides, maps_d, grad_loss_d, grad_l1_d, grad_ssim_d,
+                                grad_render_d, grad_render_l1_d, (cudaStream_t)stream);
+}
+
+int lgr_corrector_step(int64_t num_views, int64_t index, int32_t start_step, double log_lr_init, double log_lr_final,
+                       int32_t* steps_d, float* param_d, float* grad_d, float* exp_avg_d, float* exp_avg_sq_d,
+                       float* max_exp_avg_sq_d, void* stream) {
+  if (num_views < 1 || index < 0 || index >= num_views || !steps_d || !param_d || !grad_d || !exp_avg_d || !exp_avg_sq_d)
+    return LGR_E_BADARG;
+  return launch_corrector_step(index, start_step, log_lr_init, log_lr_final, steps_d, param_d, grad_d, exp_avg_d,
+                               exp_avg_sq_d, max_exp_avg_sq_d, (cudaStream_t)stream);
 }
 
 // Shapes, pointers and strides of an lgr_depth_loss_* call: the patches index all three maps at the ground truth's

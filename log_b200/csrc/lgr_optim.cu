@@ -9,6 +9,8 @@
 //                          row, then one per point_id entry; plain read-modify-writes on unique rows
 //   log_step_kernel        LoG.step (level_of_gaussian.py:379-398): every key's Adam update and the scale clamp
 //                          (:367-377), one thread per (row, float) across all keys
+//   corrector_step_kernel  Corrector.step (LoG/model/corrector.py:35-62) for one view: one warp, the step count, LoG's
+//                          skip before start_step and its learning-rate schedule on the device
 #include "lgr_common.cuh"
 #include "lgr_prof.cuh"
 
@@ -178,6 +180,79 @@ int launch_log_step(const lgr_step& s, int64_t num_leaf, int64_t num_node, const
   if (total <= 0) return 0;
   log_step_kernel<<<(unsigned)((total + ADAM_THREADS - 1) / ADAM_THREADS), ADAM_THREADS, 0, st>>>(s, num_leaf, total, leaf,
                                                                                                  node, flag_vis);
+  LGR_CHECK_LAUNCH();
+  return 0;
+}
+
+// ---- Corrector.step: one row of the (V, 3) view-correction table ----------------------------------------------------
+
+// fp64 products and sums rounded one by one, as numpy's (no contraction into a fused multiply-add).
+__device__ __forceinline__ double dmul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__device__ __forceinline__ double dadd_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
+// One warp.  steps[i] += 1 (int32 wrap); s = steps[i] - start_step; s < 0 returns (the gradient row keeps accumulating,
+// as in LoG).  Otherwise lanes 0..2 update one column each.
+//   lr = exp(log lr_init (1 - t) + log lr_final t), t = clip(s / 100, 0, 1): numpy's float64 operations in numpy's
+//     order, each rounded; the two logs come from numpy on the host.  exp is the CUDA math library's (max 1 ulp in
+//     fp64), which may differ from numpy's in the last bit of the double; lr enters as (float)lr, where that shows only
+//     if the double lies within an ulp of a float rounding boundary.
+//   The bias corrections as LoG's _single_tensor_adam computes them with a tensor step, in float32 tensor operations:
+//     1 - 0.9^s, sqrt(1 - 0.999^s) and step_size = (1 / bc1) * (float)lr (Tensor.__rtruediv__ is reciprocal() * lr).
+//   The moments as torch's CUDA kernels compute LoG's in-place ops, the rounding LoG gets when it trains on the GPU:
+//     exp_avg.mul_(b1).add_(g, alpha=1-b1) is fma(1-b1, g, m*b1) (AddFunctor a + alpha*b, contracted), and
+//     exp_avg_sq.mul_(b2).addcmul_(g, g, value=1-b2) is fma(1-b2, g*g, v*b2) (a + alpha*(b*c), contracted).  torch's
+//     CPU addcmul_ rounds the second as fma((1-b2)*g, g, v*b2) instead; adam_element rounds every product separately.
+//   AMSGrad maximum (NaN propagates, as torch.max), denominator and update in torch's order; then grad[i] = 0.
+__global__ void __launch_bounds__(32)
+corrector_step_kernel(int64_t index, int32_t start_step, double log_lr_init, double log_lr_final, int32_t* __restrict__ steps,
+                      float* __restrict__ param, float* __restrict__ grad, float* __restrict__ exp_avg,
+                      float* __restrict__ exp_avg_sq, float* __restrict__ max_exp_avg_sq) {
+  const int lane = threadIdx.x;
+  const int32_t count = (int32_t)((uint32_t)steps[index] + 1u);
+  __syncwarp();
+  if (lane == 0) steps[index] = count;
+  const int32_t s = (int32_t)((uint32_t)count - (uint32_t)start_step);
+  if (s < 0 || lane >= 3) return;
+  const double t = fmin(fmax((double)s / 100.0, 0.0), 1.0);
+  const double lr = exp(dadd_rn(dmul_rn(log_lr_init, 1.0 - t), dmul_rn(log_lr_final, t)));
+  const float sf = (float)s;
+  const float bc1 = __fsub_rn(1.f, powf(0.9f, sf)), bc2 = __fsub_rn(1.f, powf(0.999f, sf));
+  const float step_size = __fmul_rn(__fdiv_rn(1.f, bc1), (float)lr);
+  const float omb1 = (float)(1.0 - 0.9), omb2 = (float)(1.0 - 0.999);
+  const int64_t e = index * 3 + lane;
+  const float g = grad[e];
+  const float m = __fmaf_rn(omb1, g, __fmul_rn(exp_avg[e], 0.9f));
+  const float v = __fmaf_rn(omb2, __fmul_rn(g, g), __fmul_rn(exp_avg_sq[e], 0.999f));
+  exp_avg[e] = m;
+  exp_avg_sq[e] = v;
+  float vv = v;
+  if (max_exp_avg_sq) {
+    const float vm = max_exp_avg_sq[e];
+    vv = vm != vm ? vm : v != v ? v : fmaxf(vm, v);      // torch.max: NaN propagates
+    max_exp_avg_sq[e] = vv;
+  }
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vv), __fsqrt_rn(bc2)), 1e-15f);
+  param[e] = __fadd_rn(param[e], __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+  grad[e] = 0.f;
+}
+
+int launch_corrector_step(int64_t index, int32_t start_step, double log_lr_init, double log_lr_final, int32_t* steps,
+                          float* param, float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
+                          cudaStream_t st) {
+  corrector_step_kernel<<<1, 32, 0, st>>>(index, start_step, log_lr_init, log_lr_final, steps, param, grad, exp_avg,
+                                          exp_avg_sq, max_exp_avg_sq);
   LGR_CHECK_LAUNCH();
   return 0;
 }

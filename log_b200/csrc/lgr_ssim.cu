@@ -9,6 +9,14 @@
 //                       11-tap correlation, dL/dx = g (w*P0 + 2x w*P1 + y w*P2) with g = -dL/dloss / count
 // Both images are read through element strides, so LoG's channels-last ground truth and cropped render need no copy.
 // At 1920x1080x3: 50 MB of images read, 74 MB of maps written and read back, 25 MB of gradient written.
+//
+// The same three kernels with PHOTO = true are LoG's whole photometric loss (NaiveRendererAndLoss.calculate_loss,
+// renderer.py:253-266): 0.2 ssim + 0.8 l1, l1 = mean |r1 - y| with r1 LoG's render_correct or the render itself.
+//   forward    x is staged as LoG's blend y m + x (1 - m) when mask_ignore is given; each CTA also sums |r1 - y| in fp64
+//              over its 32x32 image block, and the last tile row / column over the 10-pixel remainder (its halo)
+//   reduce     ssim, l1 and loss = fl(fl(0.2 ssim) + fl(0.8 l1)) from the two rows of partials, in a fixed order
+//   backward   three upstream scalars (d/dloss, d/dl1, d/dssim) from the device; dL/dx = (SSIM term [+ l1 term when r1
+//              is the render]) (1 - m), and dL/dr1 = sign(r1 - y) dL/dl1 / numel when r1 is a separate image
 #include "lgr_common.cuh"
 
 namespace lgr {
@@ -33,6 +41,24 @@ struct SsimArgs {
   float bias;
 };
 
+// What the photometric instance (PHOTO = true) adds.  The SSIM instance ignores it.
+struct PhotoArgs {
+  const float* mask;         // (B, H, W) mask_ignore, or null: no blend
+  int64_t sm[3];             // its element strides
+  const float* r1;           // (B, C, H, W) image of the L1 term, or null: the (blended) render x
+  int64_t sr[4];             // its element strides
+  float* dr1;                // backward: contiguous (B, C, H, W) dL/dr1 (only with r1)
+  float numel_f;             // backward: (float)(B C H W), the divisor of the L1 mean
+};
+
+// LoG's blend gt * m + render * (1 - m), each torch operation rounded.
+__device__ __forceinline__ float photo_blend(float x, float y, float m) {
+  return __fadd_rn(__fmul_rn(y, m), __fmul_rn(x, __fsub_rn(1.f, m)));
+}
+
+// torch's sign: 1, -1, or 0 (also for NaN).
+__device__ __forceinline__ float photo_sign(float d) { return d > 0.f ? 1.f : d < 0.f ? -1.f : 0.f; }
+
 // Block-wide double sum in a fixed order (warp tree, then the warps in index order).  Convergent.
 __device__ __forceinline__ double ssim_block_sum(double v, double* red) {
 #pragma unroll
@@ -45,9 +71,10 @@ __device__ __forceinline__ double ssim_block_sum(double v, double* red) {
   return s;      // valid in thread 0
 }
 
+template <bool PHOTO>
 __global__ void __launch_bounds__(SSIM_THREADS)
 ssim_fwd_kernel(const SsimArgs a, const float* __restrict__ x, const float* __restrict__ y, double* __restrict__ partial,
-                float* __restrict__ maps) {
+                float* __restrict__ maps, const PhotoArgs p) {
   __shared__ float sx[SSIM_S][SSIM_S], sy[SSIM_S][SSIM_S];
   __shared__ float hm[5][SSIM_S][SSIM_T];      // horizontal pass, centred: E[x], E[y], E[x^2], E[y^2], E[(x-y)^2]
   __shared__ double red[SSIM_THREADS / 32];
@@ -63,8 +90,16 @@ ssim_fwd_kernel(const SsimArgs a, const float* __restrict__ x, const float* __re
   for (int i = threadIdx.x; i < SSIM_S * SSIM_S; i += SSIM_THREADS) {
     const int r = i / SSIM_S, q = i % SSIM_S, gy = oy0 + r, gx = ox0 + q;
     const bool in = gy < a.H && gx < a.W;
-    sx[r][q] = in ? xp[gy * a.s1[2] + gx * a.s1[3]] : 0.f;
-    sy[r][q] = in ? yp[gy * a.s2[2] + gx * a.s2[3]] : 0.f;
+    if constexpr (!PHOTO) {
+      sx[r][q] = in ? xp[gy * a.s1[2] + gx * a.s1[3]] : 0.f;
+      sy[r][q] = in ? yp[gy * a.s2[2] + gx * a.s2[3]] : 0.f;
+    } else {
+      float xv = in ? xp[gy * a.s1[2] + gx * a.s1[3]] : 0.f;
+      const float yv = in ? yp[gy * a.s2[2] + gx * a.s2[3]] : 0.f;
+      if (p.mask && in) xv = photo_blend(xv, yv, p.mask[n * p.sm[0] + gy * p.sm[1] + gx * p.sm[2]]);
+      sx[r][q] = xv;
+      sy[r][q] = yv;
+    }
   }
   __syncthreads();
   // Moments are taken about a local centre -- the horizontal pass about the middle pixel of its 11 taps, the vertical pass
@@ -125,20 +160,54 @@ ssim_fwd_kernel(const SsimArgs a, const float* __restrict__ x, const float* __re
   }
   const double s = ssim_block_sum(acc, red);
   if (threadIdx.x == 0) partial[blockIdx.x] = s;
+  if constexpr (PHOTO) {
+    // |r1 - y| over this CTA's 32x32 image block; the last tile row / column also owns the rest of the image, which its
+    // staged halo covers (the map is 10 pixels smaller than the image)
+    const int ey = ty == a.tiles_y - 1 ? a.H - oy0 : SSIM_T, ex = tx == a.tiles_x - 1 ? a.W - ox0 : SSIM_T;
+    const float* rp = p.r1 ? p.r1 + n * p.sr[0] + c * p.sr[1] : nullptr;
+    double l1 = 0.0;
+    for (int i = threadIdx.x; i < ey * ex; i += SSIM_THREADS) {
+      const int r = i / ex, q = i % ex;
+      const float rv = rp ? rp[(oy0 + r) * p.sr[2] + (ox0 + q) * p.sr[3]] : sx[r][q];
+      l1 += (double)fabsf(__fsub_rn(rv, sy[r][q]));
+    }
+    __syncthreads();      // thread 0 has read red
+    const double s1 = ssim_block_sum(l1, red);
+    if (threadIdx.x == 0) partial[gridDim.x + blockIdx.x] = s1;
+  }
 }
 
+// PHOTO: loss[0] = 0.2 ssim + 0.8 l1, loss[1] = l1, loss[2] = ssim (three separate floats: out[0..2]).
+template <bool PHOTO>
 __global__ void __launch_bounds__(SSIM_THREADS)
-ssim_reduce_kernel(const double* __restrict__ partial, int64_t blocks, double inv_count, float* __restrict__ loss) {
+ssim_reduce_kernel(const double* __restrict__ partial, int64_t blocks, double inv_count, float* __restrict__ loss,
+                   double inv_numel, float* __restrict__ l1_out, float* __restrict__ ssim_out) {
   __shared__ double red[SSIM_THREADS / 32];
   double acc = 0.0;
   for (int64_t i = threadIdx.x; i < blocks; i += SSIM_THREADS) acc += partial[i];
   const double s = ssim_block_sum(acc, red);
-  if (threadIdx.x == 0) *loss = (float)(s * inv_count);
+  if constexpr (!PHOTO) {
+    if (threadIdx.x == 0) *loss = (float)(s * inv_count);
+  } else {
+    double acc1 = 0.0;
+    for (int64_t i = threadIdx.x; i < blocks; i += SSIM_THREADS) acc1 += partial[blocks + i];
+    __syncthreads();      // thread 0 has read red
+    const double s1 = ssim_block_sum(acc1, red);
+    if (threadIdx.x == 0) {
+      const float ssim = (float)(s * inv_count), l1 = (float)(s1 * inv_numel);
+      *ssim_out = ssim;
+      *l1_out = l1;
+      *loss = __fadd_rn(__fmul_rn(0.2f, ssim), __fmul_rn(0.8f, l1));
+    }
+  }
 }
 
+// PHOTO: grad_loss[0..2] are three separate device scalars, d/dloss, d/dl1, d/dssim.
+template <bool PHOTO>
 __global__ void __launch_bounds__(SSIM_THREADS)
 ssim_bwd_kernel(const SsimArgs a, const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ maps,
-                const float* __restrict__ grad_loss, float inv_count, float* __restrict__ dx) {
+                const float* __restrict__ grad_loss, float inv_count, float* __restrict__ dx, const PhotoArgs p,
+                const float* __restrict__ grad_l1, const float* __restrict__ grad_ssim) {
   __shared__ float sp[3][SSIM_S][SSIM_S];
   __shared__ float hp[3][SSIM_S][SSIM_T];
   int64_t b = blockIdx.x;
@@ -169,7 +238,14 @@ ssim_bwd_kernel(const SsimArgs a, const float* __restrict__ x, const float* __re
     hp[0][r][q] = h0; hp[1][r][q] = h1; hp[2][r][q] = h2;
   }
   __syncthreads();
-  const float g = -grad_loss[0] * inv_count;
+  float g, gl1 = 0.f;
+  if constexpr (!PHOTO) {
+    g = -grad_loss[0] * inv_count;
+  } else {
+    // autograd of loss = 0.2 ssim + 0.8 l1 with ssim and l1 also outputs: each product rounded, then the sum
+    g = -__fadd_rn(__fmul_rn(grad_loss[0], 0.2f), grad_ssim[0]) * inv_count;
+    gl1 = __fdiv_rn(__fadd_rn(__fmul_rn(grad_loss[0], 0.8f), grad_l1[0]), p.numel_f);
+  }
   const int64_t n = plane / a.C, c = plane % a.C;
   const float* xp = x + n * a.s1[0] + c * a.s1[1];
   const float* yp = y + n * a.s2[0] + c * a.s2[1];
@@ -185,8 +261,27 @@ ssim_bwd_kernel(const SsimArgs a, const float* __restrict__ x, const float* __re
       const float w = a.w[j];
       q0 += w * hp[0][row + j][col]; q1 += w * hp[1][row + j][col]; q2 += w * hp[2][row + j][col];
     }
-    const float xv = xp[iy * a.s1[2] + ix * a.s1[3]], yv = yp[iy * a.s2[2] + ix * a.s2[3]];
-    dp[(int64_t)iy * a.W + ix] = g * (q0 + 2.f * xv * q1 + yv * q2);
+    float xv = xp[iy * a.s1[2] + ix * a.s1[3]];
+    const float yv = yp[iy * a.s2[2] + ix * a.s2[3]];
+    if constexpr (!PHOTO) {
+      dp[(int64_t)iy * a.W + ix] = g * (q0 + 2.f * xv * q1 + yv * q2);
+    } else {
+      float m = 0.f;
+      if (p.mask) {
+        m = p.mask[n * p.sm[0] + iy * p.sm[1] + ix * p.sm[2]];
+        xv = photo_blend(xv, yv, m);
+      }
+      float d = g * (q0 + 2.f * xv * q1 + yv * q2);
+      const int64_t e = plane * (int64_t)a.H * a.W + (int64_t)iy * a.W + ix;
+      if (p.r1) {
+        const float rv = p.r1[n * p.sr[0] + c * p.sr[1] + iy * p.sr[2] + ix * p.sr[3]];
+        p.dr1[e] = __fmul_rn(photo_sign(__fsub_rn(rv, yv)), gl1);
+      } else {
+        d = __fadd_rn(d, __fmul_rn(photo_sign(__fsub_rn(xv, yv)), gl1));
+      }
+      if (p.mask) d = __fmul_rn(d, __fsub_rn(1.f, m));
+      dp[(int64_t)iy * a.W + ix] = d;
+    }
   }
 }
 
@@ -222,10 +317,10 @@ int launch_ssim_fwd(int B, int C, int H, int W, const float* img1, const int64_t
   a.tiles_x = (a.Wo + SSIM_T - 1) / SSIM_T;
   a.tiles_y = (a.Ho + SSIM_T - 1) / SSIM_T;
   const int64_t blocks = (int64_t)B * C * a.tiles_x * a.tiles_y;
-  ssim_fwd_kernel<<<(unsigned)blocks, SSIM_THREADS, 0, st>>>(a, img1, img2, partial, maps);
+  ssim_fwd_kernel<false><<<(unsigned)blocks, SSIM_THREADS, 0, st>>>(a, img1, img2, partial, maps, PhotoArgs{});
   LGR_CHECK_LAUNCH();
   const double count = (double)B * C * a.Ho * a.Wo;
-  ssim_reduce_kernel<<<1, SSIM_THREADS, 0, st>>>(partial, blocks, 1.0 / count, loss);
+  ssim_reduce_kernel<false><<<1, SSIM_THREADS, 0, st>>>(partial, blocks, 1.0 / count, loss, 0.0, nullptr, nullptr);
   LGR_CHECK_LAUNCH();
   return 0;
 }
@@ -237,7 +332,53 @@ int launch_ssim_bwd(int B, int C, int H, int W, const float* img1, const int64_t
   a.tiles_y = (H + SSIM_T - 1) / SSIM_T;
   const int64_t blocks = (int64_t)B * C * a.tiles_x * a.tiles_y;
   const double count = (double)B * C * a.Ho * a.Wo;
-  ssim_bwd_kernel<<<(unsigned)blocks, SSIM_THREADS, 0, st>>>(a, img1, img2, maps, grad_loss, (float)(1.0 / count), grad_img1);
+  ssim_bwd_kernel<false><<<(unsigned)blocks, SSIM_THREADS, 0, st>>>(a, img1, img2, maps, grad_loss, (float)(1.0 / count),
+                                                                     grad_img1, PhotoArgs{}, nullptr, nullptr);
+  LGR_CHECK_LAUNCH();
+  return 0;
+}
+
+static PhotoArgs photo_args(int B, int C, int H, int W, const float* mask, const int64_t* sm, const float* r1,
+                            const int64_t* sr, float* dr1) {
+  PhotoArgs p{};
+  p.mask = mask;
+  p.r1 = r1;
+  p.dr1 = dr1;
+  for (int k = 0; k < 3; k++) p.sm[k] = mask ? sm[k] : 0;
+  for (int k = 0; k < 4; k++) p.sr[k] = r1 ? sr[k] : 0;
+  p.numel_f = (float)((double)B * C * H * W);
+  return p;
+}
+
+// render = img1, gt = img2; partial holds two rows of per-CTA sums (SSIM, then L1).
+int launch_photometric_fwd(int B, int C, int H, int W, const float* render, const int64_t* sr, const float* gt,
+                           const int64_t* sg, const float* mask, const int64_t* sm, const float* r1, const int64_t* s1,
+                           double* partial, float* loss, float* l1, float* ssim, float* maps, cudaStream_t st) {
+  SsimArgs a = ssim_args(B, C, H, W, sr, sg);
+  a.tiles_x = (a.Wo + SSIM_T - 1) / SSIM_T;
+  a.tiles_y = (a.Ho + SSIM_T - 1) / SSIM_T;
+  const int64_t blocks = (int64_t)B * C * a.tiles_x * a.tiles_y;
+  const PhotoArgs p = photo_args(B, C, H, W, mask, sm, r1, s1, nullptr);
+  ssim_fwd_kernel<true><<<(unsigned)blocks, SSIM_THREADS, 0, st>>>(a, render, gt, partial, maps, p);
+  LGR_CHECK_LAUNCH();
+  const double count = (double)B * C * a.Ho * a.Wo, numel = (double)B * C * H * W;
+  ssim_reduce_kernel<true><<<1, SSIM_THREADS, 0, st>>>(partial, blocks, 1.0 / count, loss, 1.0 / numel, l1, ssim);
+  LGR_CHECK_LAUNCH();
+  return 0;
+}
+
+int launch_photometric_bwd(int B, int C, int H, int W, const float* render, const int64_t* sr, const float* gt,
+                           const int64_t* sg, const float* mask, const int64_t* sm, const float* r1, const int64_t* s1,
+                           const float* maps, const float* grad_loss, const float* grad_l1, const float* grad_ssim,
+                           float* grad_render, float* grad_r1, cudaStream_t st) {
+  SsimArgs a = ssim_args(B, C, H, W, sr, sg);
+  a.tiles_x = (W + SSIM_T - 1) / SSIM_T;
+  a.tiles_y = (H + SSIM_T - 1) / SSIM_T;
+  const int64_t blocks = (int64_t)B * C * a.tiles_x * a.tiles_y;
+  const double count = (double)B * C * a.Ho * a.Wo;
+  const PhotoArgs p = photo_args(B, C, H, W, mask, sm, r1, s1, grad_r1);
+  ssim_bwd_kernel<true><<<(unsigned)blocks, SSIM_THREADS, 0, st>>>(a, render, gt, maps, grad_loss, (float)(1.0 / count),
+                                                                    grad_render, p, grad_l1, grad_ssim);
   LGR_CHECK_LAUNCH();
   return 0;
 }

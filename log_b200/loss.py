@@ -6,7 +6,11 @@
 strides (LoG's permuted ground truth and cropped render need no copy) and never synchronise with the host.
 
 `append_depth_loss` is a drop-in for NaiveRendererAndLoss.append_depth_loss (renderer.py:268-292), LoG's depth-supervision
-loss; `depth_patch_loss` and `depth_vis` are its two parts for explicit patch corners (kernels in lgr_depth_loss.cu)."""
+loss; `depth_patch_loss` and `depth_vis` are its two parts for explicit patch corners (kernels in lgr_depth_loss.cu).
+
+`calculate_loss` is a drop-in for NaiveRendererAndLoss.calculate_loss (renderer.py:253-266), LoG's photometric loss with its
+mask blend and view-corrected L1 term; `photometric_loss` is the same computation on explicit tensors (`lgr_photometric_*`,
+the photometric instance of the SSIM kernels)."""
 import ctypes
 import math
 
@@ -226,3 +230,109 @@ def append_depth_loss(self, gt_depth, pred_depth, output):
     output['loss_dict']['depth'] = depth_loss
     output['loss'] += 1. * depth_loss
     return output
+
+
+# ---- photometric loss (LoG's calculate_loss) -------------------------------------------------------------------------
+
+def _strides3(t):
+    return (ctypes.c_int64 * 3)(*t.stride())
+
+
+def _photo_args(render, gt, render_l1, mask):
+    B, C, H, W = render.shape
+    return (B, C, H, W, _ptr(render), _strides(render), _ptr(gt), _strides(gt),
+            None if mask is None else _ptr(mask), None if mask is None else _strides3(mask),
+            None if render_l1 is None else _ptr(render_l1), None if render_l1 is None else _strides(render_l1))
+
+
+def _photo_forward(render, gt, render_l1, mask, want_maps):
+    """-> (loss, l1, ssim, maps or None)."""
+    B, C, H, W = render.shape
+    dev = render.device
+    scratch = torch.empty(_capi.photo_scratch_doubles(B, C, H, W), dtype=torch.float64, device=dev)
+    loss, l1, ssim = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(3))
+    maps = torch.empty(_capi.ssim_map_floats(B, C, H, W), dtype=torch.float32, device=dev) if want_maps else None
+    _capi.check(_capi.load().lgr_photometric_forward(*_photo_args(render, gt, render_l1, mask), _ptr(scratch), _ptr(loss),
+                                                     _ptr(l1), _ptr(ssim), None if maps is None else _ptr(maps),
+                                                     _capi.current_stream(dev)), 'lgr_photometric_forward')
+    return loss, l1, ssim, maps
+
+
+class _PhotometricLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, render, gt, render_l1, mask):
+        loss, l1, ssim, maps = _photo_forward(render, gt, render_l1, mask, True)
+        ctx.save_for_backward(render, gt, render_l1, mask, maps)
+        return loss, l1, ssim
+
+    @staticmethod
+    def backward(ctx, grad_loss, grad_l1, grad_ssim):
+        render, gt, render_l1, mask, maps = ctx.saved_tensors
+        dev = render.device
+        grads = [g.to(torch.float32).contiguous() for g in (grad_loss, grad_l1, grad_ssim)]
+        grad_render = torch.empty(render.shape, dtype=torch.float32, device=dev)
+        grad_l1_img = None if render_l1 is None else torch.empty(render_l1.shape, dtype=torch.float32, device=dev)
+        _capi.check(_capi.load().lgr_photometric_backward(*_photo_args(render, gt, render_l1, mask), _ptr(maps),
+                                                          *(_ptr(g) for g in grads), _ptr(grad_render),
+                                                          None if grad_l1_img is None else _ptr(grad_l1_img),
+                                                          _capi.current_stream(dev)), 'lgr_photometric_backward')
+        return grad_render, None, grad_l1_img, None
+
+
+def photometric_loss(render, gt, render_l1=None, mask_ignore=None):
+    """LoG's photometric loss, `0.2 * ssim + 0.8 * l1`, as three 0-d float32 tensors `(loss, l1, ssim)` on the device.
+
+    render, gt: float32 (B, C, H, W) on one CUDA device, H and W >= 11, read through their strides (LoG's channels-last
+    ground truth and MaskForeground's crop are not copied).  With `mask_ignore` (float32 (B, H, W), any strides), the
+    SSIM term and -- when `render_l1` is None -- the L1 term see LoG's blend `gt * m + render * (1 - m)`.  `render_l1`
+    (float32 (B, C, H, W), e.g. LoG's `render_correct[:, :3]`) is the image of the L1 term, read unblended as LoG does.
+    `ssim` is SSIM(11, C)'s loss of the (blended) render, `l1 = mean |render_l1 - gt|`; both sums are in fp64 in a fixed
+    order, so the results repeat bit for bit.  The gradient flows to `render` and `render_l1`; gt and the mask take
+    none.  Never synchronises with the host."""
+    for t, name in ((render, 'render'), (gt, 'gt')) + (() if render_l1 is None else ((render_l1, 'render_l1'),)) + \
+            (() if mask_ignore is None else ((mask_ignore, 'mask_ignore'),)):
+        _capi.require_cuda(t, name)
+        if t.dtype != torch.float32:
+            raise TypeError(f'photometric_loss: {name} must be float32, got {t.dtype}')
+    if render.dim() != 4 or render.shape != gt.shape:
+        raise ValueError(f'photometric_loss: render {tuple(render.shape)} and gt {tuple(gt.shape)} must be the same '
+                         '(B, C, H, W)')
+    B, C, H, W = render.shape
+    if render_l1 is not None and render_l1.shape != render.shape:
+        raise ValueError(f'photometric_loss: render_l1 {tuple(render_l1.shape)} must match render {tuple(render.shape)}')
+    if mask_ignore is not None and tuple(mask_ignore.shape) != (B, H, W):
+        raise ValueError(f'photometric_loss: mask_ignore {tuple(mask_ignore.shape)} must be ({B}, {H}, {W})')
+    if H < _capi.LGR_SSIM_WINDOW or W < _capi.LGR_SSIM_WINDOW or B < 1:
+        raise ValueError(f'photometric_loss: images of {H}x{W} are smaller than the SSIM window')
+    if len({t.device for t in (render, gt, render_l1, mask_ignore) if t is not None}) != 1:
+        raise ValueError('photometric_loss: every input must be on the same device')
+    if gt.requires_grad or (mask_ignore is not None and mask_ignore.requires_grad):
+        raise NotImplementedError('photometric_loss: gt and mask_ignore take no gradient')
+    mask = None if mask_ignore is None else mask_ignore.detach()
+    if torch.is_grad_enabled() and (render.requires_grad or (render_l1 is not None and render_l1.requires_grad)):
+        return _PhotometricLoss.apply(render, gt, render_l1, mask)
+    return _photo_forward(render, gt, render_l1, mask, False)[:3]
+
+
+def calculate_loss(self, gt_image, render, output, mask_ignore=None):
+    """Drop-in for LoG's NaiveRendererAndLoss.calculate_loss (renderer.py:253-266), bound to the renderer:
+
+        renderer.calculate_loss = types.MethodType(log_b200.loss.calculate_loss, renderer)
+
+    `photometric_loss(render, gt_image, output['render_correct'][:, :3] if present, mask_ignore)`: the mask blend, the
+    SSIM term on the blended render, the L1 term on LoG's view-corrected render when there is one (unblended, as in
+    LoG), `output['loss'] = 0.2 * ssim + 0.8 * l1`, in three launches forward and one backward, with no host read.
+    The renderer's `ssim_loss` must be an 11x11 SSIM (LoG's module or log_b200.loss.SSIM) and its `l1_loss` a mean
+    nn.L1Loss; anything else raises NotImplementedError.
+
+    Divergence: `output['loss_dict']['l1']` and `['ssim']` are 0-d device tensors, not Python floats, because reading
+    them would synchronise with the host between the forward and the backward.  LoG's trainer only logs them."""
+    ssim_loss, l1_loss = getattr(self, 'ssim_loss', None), getattr(self, 'l1_loss', None)
+    if getattr(ssim_loss, 'window_size', None) != _capi.LGR_SSIM_WINDOW or not isinstance(ssim_loss, torch.nn.Module):
+        raise NotImplementedError(f'calculate_loss: ssim_loss {type(ssim_loss).__name__} is not an SSIM with an 11x11 window')
+    if not isinstance(l1_loss, torch.nn.L1Loss) or l1_loss.reduction != 'mean':
+        raise NotImplementedError(f'calculate_loss: l1_loss {l1_loss!r} is not a mean nn.L1Loss')
+    render_l1 = output['render_correct'][:, :3] if 'render_correct' in output.keys() else None
+    loss, l1, ssim = photometric_loss(render, gt_image, render_l1, mask_ignore)
+    output['loss_dict'] = {'l1': l1, 'ssim': ssim}
+    output['loss'] = loss

@@ -6,7 +6,8 @@ as one in-place kernel, without the `index.cpu()` synchronisation (:168).
 
 `counter_update_by_output` and `log_step` are drop-ins for the two calls LoG's training step makes after
 `loss.backward()` (LoG/utils/trainer.py:159-160): Counter.update_by_output and LoG.step, on `lgr_counter_update` and
-`lgr_log_step`."""
+`lgr_log_step`.  `corrector_step` is a drop-in for Corrector.step, the per-view colour correction LoG.step runs last
+(`lgr_corrector_step`)."""
 import ctypes
 import math
 
@@ -148,8 +149,9 @@ def log_step(self):
     `sparse_adam_step_` (bit for bit) on the row of the parameter table and its optimiser state, then `scaling` clamped
     to [log radius3d_min, log radius3d_max] (torch.clamp semantics; applied also when `scaling` has no gradient).
     Learning rates (LoG's own schedulers), `1 - beta1^step` and `sqrt(1 - beta2^step)` are computed on the host in
-    Python floats, as LoG does.  `optimizer.xyz_lr`, `self.lr`, the base-iteration message and LoG's own view
-    correction (`self.view_correction.step()`) follow LoG.
+    Python floats, as LoG does.  `optimizer.xyz_lr`, `self.lr` and the base-iteration message follow LoG.  After
+    `base_iter` it calls `self.view_correction.step()` as LoG does; bind `corrector_step` there (below) so that this
+    call, too, runs on the device without a host read.
 
     Synchronisation: `optimizer.global_steps` is read once, on the first call (and again only if something else changed
     it since, e.g. `load_state_dict`); afterwards the step never reads the device.  The Gaussians of the flagged rows
@@ -224,3 +226,50 @@ def log_step(self):
         print(f'[{self.__class__.__name__}] base iteration {self.base_iter} done, enable view_correction module')
     if self.use_view_correction and step > self.base_iter:
         self.view_correction.step()
+
+
+# ---- LoG's per-view colour correction: Corrector.step ----------------------------------------------------------------
+
+def corrector_step(self):
+    """Drop-in for LoG's Corrector.step (LoG/model/corrector.py:35-62), bound to the model's corrector:
+
+        model.view_correction.step = types.MethodType(log_b200.optim.corrector_step, model.view_correction)
+
+    One `lgr_corrector_step` launch and no host read: for the view `self.index` (set by `Corrector.__getitem__` in
+    LoG's render), `steps += 1`; from `start_step` on, the AMSGrad Adam update of the `(1, 3)` row with LoG's learning
+    rate schedule (in fp64) and LoG's float32 tensor bias corrections, then the gradient row is zeroed.  Before
+    `start_step` the row's gradient keeps accumulating, as in LoG.  Returns 0 when view correction is off, as LoG does,
+    and None otherwise.  Raises ValueError when `self.index` is None, the gradient is missing, or the parameter, its
+    gradient or the optimiser state is not a contiguous float32 (int32 for the step counts) tensor on the parameter's
+    device; IndexError for an index outside the table."""
+    if not self.use_view_correction:
+        return 0
+    if self.index is None:
+        raise ValueError('corrector_step: Corrector.index is None (no view was selected since the last step)')
+    param = self.view_correction
+    _capi.require_cuda(param, 'view_correction')
+    device = param.device
+    if param.grad is None:
+        raise ValueError('corrector_step: view_correction has no gradient')
+    opt = self.optimizer
+    tables = [param.data, param.grad] + [getattr(opt, name)['view_correction'] for name in ('exp_avg', 'exp_avg_sq')]
+    names = ['view_correction', 'view_correction.grad', 'exp_avg', 'exp_avg_sq']
+    if getattr(opt, 'use_amsgrad', False):
+        tables.append(opt.max_exp_avg_sq['view_correction'])
+        names.append('max_exp_avg_sq')
+    V = int(param.shape[0])
+    for t, name in zip(tables, names):
+        _table(t, f'Corrector {name}', device)
+        if tuple(t.shape) != (V, 3):
+            raise ValueError(f'corrector_step: {name} must be ({V}, 3), got {tuple(t.shape)}')
+    steps = opt.steps['view_correction']
+    if steps.device != device or steps.dtype != torch.int32 or not steps.is_contiguous() or tuple(steps.shape) != (V,):
+        raise ValueError(f'corrector_step: steps must be a contiguous int32 ({V},) tensor on {device}')
+    index = int(self.index)
+    if not -V <= index < V:
+        raise IndexError(f'corrector_step: index {index} is out of range for {V} views')
+    index %= V
+    ptrs = [_ptr(t) for t in tables] + [None] * (5 - len(tables))
+    _capi.check(_capi.load().lgr_corrector_step(V, index, int(self.start_step), float(np.log(self.lr_init)),
+                                                float(np.log(self.lr_final)), _ptr(steps), *ptrs,
+                                                _capi.current_stream(device)), 'lgr_corrector_step')
