@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from . import _capi
+from .rasterizer import _ptr
 
 
 def sparse_adam_step_(param, grad, exp_avg, exp_avg_sq, index, step, lr, max_exp_avg_sq=None, beta1=0.9, beta2=0.999,
@@ -32,8 +33,7 @@ def sparse_adam_step_(param, grad, exp_avg, exp_avg_sq, index, step, lr, max_exp
     c = int(param[0].numel()) if param.shape[0] else 1
     if tuple(grad.shape) != (k,) + tuple(param.shape[1:]):
         raise ValueError(f'grad shape {tuple(grad.shape)} does not match ({k},) + {tuple(param.shape[1:])}')
-    p = lambda t: None if t is None or t.numel() == 0 else ctypes.c_void_p(t.data_ptr())
-    _capi.check(lib.lgr_sparse_adam(k, c, p(index), p(grad), p(param), p(exp_avg), p(exp_avg_sq), p(max_exp_avg_sq),
+    _capi.check(lib.lgr_sparse_adam(k, c, _ptr(index), _ptr(grad), _ptr(param), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(max_exp_avg_sq),
                                     int(step), float(lr), float(beta1), float(beta2), float(eps),
                                     _capi.current_stream()), 'lgr_sparse_adam')
     return param
@@ -44,10 +44,6 @@ def sparse_adam_step_(param, grad, exp_avg, exp_avg_sq, index, step, lr, max_exp
 _COUNTER = (('create_steps', torch.int32), ('visible_count', torch.int16), ('weights_max', torch.float32),
             ('weights_sum', torch.float32), ('radii_max', torch.int16), ('area_sum', torch.int32),
             ('grad_sum', torch.float32), ('radii_max_max', torch.int32))
-
-
-def _ptr(t):
-    return None if t is None or t.numel() == 0 else ctypes.c_void_p(t.data_ptr())
 
 
 def _rows(leaf, node):

@@ -13,13 +13,9 @@ import torch
 
 from . import _capi
 from ._capi import LGR_FILTER_MAX
-from .rasterizer import FLAVOUR_FORK, rasterize_forward
+from .rasterizer import FLAVOUR_FORK, _ptr, rasterize_forward
 
 PADDING = 0.5      # LoG's padding in both branches of prepare (level_of_gaussian.py:94, :229)
-
-
-def _ptr(t):
-    return None if t is None or t.numel() == 0 else ctypes.c_void_p(t.data_ptr())
 
 
 def _table(t, name):

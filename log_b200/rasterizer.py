@@ -26,7 +26,6 @@ import torch.nn as nn
 from . import _capi
 from ._capi import LGR_FILTER_ADD, LGR_FILTER_MAX, LGR_FILTER_NONE, LgrView
 
-PREZERO_DSPLAT = bool(int(__import__('os').environ.get('LGR_PREZERO_DSPLAT', '0')))      # see rasterize_forward
 # the forward blend lists the entries some pixel composited, with their sub-tiles; the backward stages and walks only those (A/B knob)
 CONTRIB_BITS = bool(int(__import__('os').environ.get('LGR_CONTRIB_BITS', '1')))
 FLAVOUR_STOCK = 'stock'   # diff_gaussian_rasterization            (graphdeco-inria)   -> 2-tuple, cov += 0.3
@@ -155,20 +154,120 @@ def use_contrib_lists(D, max_tile_len):
     return CONTRIB_BITS and D > 0 and (max_tile_len is None or max_tile_len <= _capi.LGR_CONTRIB_MAX_LIST)
 
 
+def decode_meta(m):
+    """The LGR_META_INTS ints of meta_d, as the caller read them, as a dict: num_instances (D, the (Gaussian, tile) pairs
+    binned), max_tile_len, stock_instances (D by the stock rule, 64-bit over two words), num_visible, num_long_tiles
+    (lists longer than the shared-memory sort) and overflow (device-sized calls only: bit 0, the view outgrew its
+    buffers; bit 1, a tile list is longer than LGR_CONTRIB_MAX_LIST entries)."""
+    return dict(num_instances=int(m[0]), max_tile_len=int(m[1]), stock_instances=(m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32),
+                num_visible=int(m[4]), num_long_tiles=int(m[5]), overflow=int(m[6]))
+
+
+def _fresh(dev):
+    """The allocator of the stages below for calls that keep nothing between steps: a new tensor per request."""
+    return lambda name, shape, dtype: torch.empty(shape, dtype=dtype, device=dev)
+
+
+def _view_tiles(view):
+    """Tiles in the rows `view` renders (tile_row_end = 0: all rows)."""
+    gx, gy = (view.image_width + 15) // 16, (view.image_height + 15) // 16
+    return gx * (view.tile_row_end - view.tile_row_begin if view.tile_row_end else gy)
+
+
+def project(view, n, alloc, means3D, opacities, scales, rotations, colors_precomp, shs):
+    """The forward's first stage, lgr_forward_project of n Gaussians into `view`.  Buffers come from alloc(name, shape,
+    dtype), except radii, which callers return to their own callers and so is always a fresh tensor.  Returns (splat,
+    radii, clamped (SH only), tile_start, tile_cursor, meta)."""
+    ntiles = _view_tiles(view)
+    splat = alloc('splat', (n, _capi.LGR_SPLAT_FLOATS), torch.float32)
+    radii = torch.empty((n,), dtype=torch.int32, device=means3D.device)
+    clamped = alloc('clamped', (n,), torch.uint8) if shs is not None else None
+    tile_start = alloc('project_tile_start', (ntiles + 1,), torch.int32)
+    tile_cursor = alloc('project_tile_cursor', (_capi.LGR_TILE_SCRATCH_INTS * max(ntiles, 1),), torch.int32)
+    meta = alloc('project_meta', (_capi.LGR_META_INTS,), torch.int32)
+    _capi.check(_capi.load().lgr_forward_project(ctypes.byref(view), n, _ptr(means3D), _ptr(opacities), _ptr(scales), _ptr(rotations),
+                                                 _ptr(colors_precomp), _ptr(shs), _ptr(splat), _ptr(radii), _ptr(clamped),
+                                                 _ptr(tile_start), _ptr(tile_cursor), _ptr(meta), _stream(means3D.device)),
+                'lgr_forward_project')
+    return splat, radii, clamped, tile_start, tile_cursor, meta
+
+
+def render(view, n, splat, radii, tile_start, tile_cursor, meta, image, final_T, n_contrib, pid, pwp, pw, pc, alloc,
+           capacity=None, stats=None):
+    """The forward's second stage: bin, sort and blend the n projected records into the caller's outputs (image, final_T,
+    n_contrib and, with want_aux, pid, pwp, pw, pc).  A device-sized call (lgr_forward_render_device_sized) when
+    `capacity` is given: room for that many instances, nothing read back.  Otherwise host-sized (lgr_forward_render),
+    sized by `stats`, decode_meta() of the meta_d the caller read after the projection.  The instance buffers and the
+    contribution lists come from alloc(name, shape, dtype); `view` is pointed at the lists.  Returns (sorted_ids, the
+    contribution lists or None)."""
+    lib = _capi.load()
+    ntiles = _view_tiles(view)
+    if capacity:
+        D, max_len = int(capacity), None
+    else:
+        D, max_len = stats['num_instances'], stats['max_tile_len']
+        if D < 0 or stats['stock_instances'] > 0x7fffffff:      # the per-tile counters and list offsets are 32-bit
+            raise _capi.LgrError(f'this view needs {stats["stock_instances"]} (Gaussian, tile) instances by the stock rule '
+                                 f'(D = {D & 0xffffffff} binned, {stats["num_visible"]} of {n} Gaussians visible, longest tile '
+                                 f'list {max_len}): more than 2^31 - 1 is unsupported')
+    inst_key = alloc('inst_key', (D,), torch.int32)
+    inst_val = alloc('inst_val', (D,), torch.int32)
+    # the binning's staging buffer, then the sort's scratch for lists beyond shared memory
+    inst_tmp = alloc('inst_tmp', (2 * D,), torch.int32)
+    sorted_ids = alloc('sorted_ids', (D,), torch.int32)
+    # forward -> backward: the entries some pixel composited (lgr_view.contrib_*); the backward stages only those and
+    # stops a pixel after its last contributor
+    contrib = alloc('contrib', (2 * D + ntiles,), torch.int32) if use_contrib_lists(D, max_len) else None
+    set_contrib_lists(view, contrib, D, n_contrib)
+    buffers = (_ptr(splat), _ptr(radii), _ptr(tile_start), _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp),
+               _ptr(sorted_ids), _ptr(image), _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp), _ptr(pw), _ptr(pc),
+               _stream(image.device))
+    if capacity:
+        _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(view), n, D, _ptr(meta), *buffers),
+                    'lgr_forward_render_device_sized')
+    else:
+        _capi.check(lib.lgr_forward_render(ctypes.byref(view), n, D, max_len, stats['num_long_tiles'], *buffers), 'lgr_forward_render')
+    return sorted_ids, contrib
+
+
+def backward_per_gaussian(view, n, num_instances, params, splat, radii, clamped, tile_start, sorted_ids, image, grad_image, dsplat):
+    """lgr_backward with dense outputs: the blend backward over the num_instances sorted instances (none: 0, the
+    accumulator rows dsplat already hold the 2D gradients), then the per-Gaussian backward of the n Gaussians.
+    params = (means3D, opacities, scales, rotations, colors_precomp, shs) as the forward took them.  Returns
+    ((dmeans3D, dmeans2D, dopacities, dscales, drotations, dcolors, dshs), dcov3D): with cov3D_precomp (scales None,
+    view.cov3D_precomp_d set) the covariance gradient replaces the scale and rotation gradients."""
+    means3D, opacities, scales, rotations, colors_precomp, shs = params
+    f32 = dict(dtype=torch.float32, device=means3D.device)
+    cov = scales is None
+    dmeans3D, dmeans2D, dopac = torch.empty((n, 3), **f32), torch.empty((n, 3), **f32), torch.empty((n,), **f32)
+    dscales = None if cov else torch.empty((n, 3), **f32)
+    drot = None if cov else torch.empty((n, 4), **f32)
+    dcov3D = torch.empty((n, 6), **f32) if cov else None
+    if cov:
+        view.dcov3D_d = dcov3D.data_ptr()
+    # one gradient per colour channel the Gaussians carry: 3, or 6 for a six-channel colors_precomp (log_depth's
+    # generated channels 3..5 take none)
+    dcolors = torch.empty((n, int(colors_precomp.shape[-1])), **f32) if colors_precomp is not None else None
+    dshs = torch.empty((n,) + tuple(shs.shape[1:]), **f32) if shs is not None else None
+    _capi.check(_capi.load().lgr_backward(ctypes.byref(view), n, num_instances, _ptr(means3D), _ptr(opacities), _ptr(scales),
+                                          _ptr(rotations), _ptr(colors_precomp), _ptr(shs), _ptr(splat), _ptr(radii),
+                                          _ptr(clamped), _ptr(tile_start), _ptr(sorted_ids), _ptr(image), _ptr(grad_image),
+                                          _ptr(dsplat), _ptr(dmeans3D), _ptr(dmeans2D), _ptr(dopac), _ptr(dscales), _ptr(drot),
+                                          _ptr(dcolors), _ptr(dshs), None, None, 0, 0, _stream(means3D.device)), 'lgr_backward')
+    return (dmeans3D, dmeans2D, dopac, dscales, drot, dcolors, dshs), dcov3D
+
+
 class RasterState:
     """Buffers produced by the forward and consumed by the backward (kept alive by autograd)."""
     __slots__ = ('view', 'keep', 'n', 'num_instances', 'max_tile_len', 'stock_instances', 'num_visible', 'splat',
                  'radii', 'clamped', 'tile_start', 'sorted_ids', 'final_T', 'n_contrib', 'image', 'sh', 'num_owners',
-                 'band_ids', 'band_count', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D', 'contrib',
-                 'channels', 'splat_ext', 'log_depth')
+                 'dsplat', 'band_counts_host', 'point_count', 'meta', 'cov3D', 'dcov3D', 'contrib', 'splat_ext')
 
     def read_stats(self):
-        """Counters of this forward, read back from meta_d (synchronises): D, longest tile list, D by the stock rule, visible
-        Gaussians, and `overflow` (non-zero only after a device-sized call whose view outgrew its buffers, bit 0, or held a
-        tile list longer than LGR_CONTRIB_MAX_LIST entries, bit 1: outputs invalid, redo the view host-sized)."""
-        m = self.meta.tolist()
-        return dict(num_instances=int(m[0]), max_tile_len=int(m[1]), stock_instances=(m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32),
-                    num_visible=int(m[4]), overflow=int(m[6]))
+        """Counters of this forward, read back from meta_d (synchronises): decode_meta()'s dict.  `overflow` is non-zero
+        only after a device-sized call whose view outgrew its buffers or held a tile list longer than LGR_CONTRIB_MAX_LIST
+        entries: its outputs are invalid, redo the view host-sized."""
+        return decode_meta(self.meta.tolist())
 
     def contrib_lists(self):
         """The compacted contribution lists the forward wrote for the backward (lgr_view.contrib_*), as int32 views:
@@ -181,8 +280,8 @@ class RasterState:
 
 
 def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_precomp, shs, filter_mode, want_aux,
-                      tile_rows=None, num_owners=0, raw_params=False, prezero_dsplat=None, gather_index=None,
-                      instance_capacity=None, cov3D_precomp=None, log_depth=False):
+                      tile_rows=None, num_owners=0, raw_params=False, gather_index=None, instance_capacity=None,
+                      cov3D_precomp=None, log_depth=False):
     """Run the forward through the C ABI.  Returns (image, radii, pid, pwp, point_weight, state).
     num_owners > 0 (multi-GPU band mode, see log_b200/sharded.py): also compact the ids of the Gaussians reaching the
     band `tile_rows`, grouped by owner rank; the backward then returns packed gradient rows instead of dense tensors.
@@ -203,7 +302,6 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     if log_depth:      # the blend composites channels 3..5 over bg[3:6]: LoG's second call uses the same background
         bg3 = settings.bg.reshape(-1)[:3]
         settings = settings._replace(bg=torch.cat([bg3, bg3]))
-    lib = _capi.load()
     dev = means3D.device
     if cov3D_precomp is not None and (raw_params or num_owners > 0):
         raise _capi.LgrError('cov3D_precomp is not available with raw_params or in band mode')
@@ -222,44 +320,26 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         keep.append(gather_index)
         n = int(gather_index.shape[0])
     K = 0 if shs is None else int(shs.shape[1])
+    i32 = dict(dtype=torch.int32, device=dev)
+    f32 = dict(dtype=torch.float32, device=dev)
     band_ids = band_count = band_blk = band_rows = band_dsplat = None
-    # prezero_dsplat: decided by the caller (GaussianRasterizer.forward looks at requires_grad BEFORE entering the autograd
-    # function, where grad mode is always off); None = direct callers: follow the LGR_PREZERO_DSPLAT knob
-    if prezero_dsplat is None:
-        prezero_dsplat = PREZERO_DSPLAT and torch.is_grad_enabled()
-    if num_owners == 0 and prezero_dsplat:
-        # experiment (LGR_PREZERO_DSPLAT=1): the binning kernel zeroes the accumulator rows the backward will read, instead of a
-        # 48 N-byte memset at the start of the backward
-        band_dsplat = torch.empty((max(n, 1), _capi.LGR_GRAD_FLOATS), dtype=torch.float32, device=dev)
     if num_owners > 0:
-        band_rows = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
-        band_dsplat = torch.empty((max(n, 1), _capi.LGR_GRAD_FLOATS), dtype=torch.float32, device=dev)
+        band_rows = torch.empty((max(n, 1),), **i32)
+        # the backward's accumulator rows: the binning kernel zeroes the ones the backward reads
+        band_dsplat = torch.empty((max(n, 1), _capi.LGR_GRAD_FLOATS), **f32)
         nb = (n + 255) // 256
-        band_ids = torch.empty((max(256 * nb, 1),), dtype=torch.int32, device=dev)
-        band_blk = torch.empty((2 * nb + 1,), dtype=torch.int32, device=dev)
-        band_count = torch.empty((num_owners,), dtype=torch.int32, device=dev)
-    splat_ext = torch.empty((max(n, 1), 4), dtype=torch.float32, device=dev) if channels == 6 else None      # never NULL
+        band_ids = torch.empty((max(256 * nb, 1),), **i32)
+        band_blk = torch.empty((2 * nb + 1,), **i32)
+        band_count = torch.empty((num_owners,), **i32)
+        keep.extend([band_ids, band_blk, band_rows, band_count])
+    splat_ext = torch.empty((max(n, 1), 4), **f32) if channels == 6 else None      # never NULL
     keep.append(splat_ext)
     view = _make_view(settings, filter_mode, want_aux, K, tile_rows, keep, num_owners, band_ids, band_count, band_blk, band_rows, band_dsplat,
                       raw_params, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext, log_depth=log_depth)
+    alloc = _fresh(dev)
+    splat, radii, clamped, tile_start, tile_cursor, meta = project(view, n, alloc, means3D, opacities, scales, rotations,
+                                                                   colors_precomp, shs)
     H, W = view.image_height, view.image_width
-    gx, gy = (W + 15) // 16, (H + 15) // 16
-    rows = gy if tile_rows is None else int(tile_rows[1]) - int(tile_rows[0])
-    ntiles = gx * rows
-    i32 = dict(dtype=torch.int32, device=dev)
-    f32 = dict(dtype=torch.float32, device=dev)
-    splat = torch.empty((n, _capi.LGR_SPLAT_FLOATS), **f32)
-    radii = torch.empty((n,), **i32)
-    clamped = torch.empty((n,), dtype=torch.uint8, device=dev) if shs is not None else None
-    tile_start = torch.empty((ntiles + 1,), **i32)
-    tile_cursor = torch.empty((_capi.LGR_TILE_SCRATCH_INTS * max(ntiles, 1),), **i32)
-    meta = torch.empty((_capi.LGR_META_INTS,), **i32)
-    st = _stream(dev)
-    _capi.check(lib.lgr_forward_project(ctypes.byref(view), n, _ptr(means3D), _ptr(opacities), _ptr(scales),
-                                        _ptr(rotations), _ptr(colors_precomp), _ptr(shs), _ptr(splat), _ptr(radii),
-                                        _ptr(clamped), _ptr(tile_start), _ptr(tile_cursor), _ptr(meta), st),
-                'lgr_forward_project')
-    u32 = dict(dtype=torch.int32, device=dev)
     # a sharded call owns only its rows; untouched rows stay zero so that ranks can be summed
     image = torch.empty((channels, H, W), **f32) if tile_rows is None else torch.zeros((channels, H, W), **f32)
     final_T = torch.empty((H, W), **f32) if tile_rows is None else torch.ones((H, W), **f32)
@@ -270,51 +350,30 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         pid = torch.empty((H, W), **i32) if tile_rows is None else torch.full((H, W), -1, **i32)
         pwp = torch.empty((H, W), **f32) if tile_rows is None else torch.zeros((H, W), **f32)
         pw = torch.zeros((n,), **f32)
+    m = stats = None
     if instance_capacity:
         if num_owners > 0:
             raise _capi.LgrError('instance_capacity (device-sized call) is not available in band mode')
-        D, max_len, num_long, stock_D, m = int(instance_capacity), None, None, None, None
-        inst_key, inst_val = torch.empty((D,), **u32), torch.empty((D,), **u32)
-        inst_tmp = torch.empty((2 * D,), **u32)      # the binning's staging buffer
-        sorted_ids = torch.empty((D,), **i32)
-        contrib = torch.empty((2 * D + ntiles,), **i32) if use_contrib_lists(D, None) else None
-        keep.append(contrib)
-        set_contrib_lists(view, contrib, D, n_contrib)
-        _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(view), n, D, _ptr(meta), _ptr(splat), _ptr(radii), _ptr(tile_start),
-                                                        _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp), _ptr(sorted_ids), _ptr(image),
-                                                        _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp), _ptr(pw), _ptr(pc), st),
-                    'lgr_forward_render_device_sized')
     else:
         m = (meta if band_count is None else torch.cat([meta, band_count])).tolist()   # the one host sync of the forward
-        D, max_len, num_long = int(m[0]), int(m[1]), int(m[5])
-        stock_D = (m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32)
-        if D < 0 or stock_D > 0x7fffffff:      # the per-tile counters and list offsets are 32-bit
-            raise _capi.LgrError(f'this view needs {stock_D} (Gaussian, tile) instances by the stock rule (D = {m[0] & 0xffffffff} binned, '
-                                 f'{m[4]} of {n} Gaussians visible, longest tile list {max_len}): more than 2^31 - 1 is unsupported')
-        inst_key = torch.empty((D,), **u32)
-        inst_val = torch.empty((D,), **u32)
-        inst_tmp = torch.empty((2 * D,), **u32)      # the binning's staging buffer, then the sort's scratch for lists beyond shared memory
-        sorted_ids = torch.empty((D,), **i32)
-        # forward -> backward: the entries some pixel composited (lgr_view.contrib_*); the backward stages only those and
-        # stops a pixel after its last contributor
-        contrib = torch.empty((2 * D + ntiles,), **i32) if use_contrib_lists(D, max_len) else None
-        keep.append(contrib)
-        set_contrib_lists(view, contrib, D, n_contrib)
-        _capi.check(lib.lgr_forward_render(ctypes.byref(view), n, D, max_len, num_long, _ptr(splat), _ptr(radii), _ptr(tile_start),
-                                           _ptr(tile_cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp),
-                                           _ptr(sorted_ids), _ptr(image), _ptr(final_T), _ptr(n_contrib), _ptr(pid),
-                                           _ptr(pwp), _ptr(pw), _ptr(pc), st), 'lgr_forward_render')
+        stats = decode_meta(m)
+    sorted_ids, contrib = render(view, n, splat, radii, tile_start, tile_cursor, meta, image, final_T, n_contrib, pid, pwp, pw, pc,
+                                 alloc, instance_capacity, stats)
+    keep.append(contrib)
     s = RasterState()
-    s.view, s.keep, s.n, s.num_instances, s.max_tile_len = view, keep, n, D, max_len
-    s.stock_instances, s.num_visible = stock_D, (int(m[4]) if m is not None else None)
-    s.meta = meta
+    s.view, s.keep, s.n, s.meta = view, keep, n, meta
+    if stats is None:
+        s.num_instances, s.max_tile_len, s.stock_instances, s.num_visible = int(instance_capacity), None, None, None
+    else:
+        s.num_instances, s.max_tile_len = stats['num_instances'], stats['max_tile_len']
+        s.stock_instances, s.num_visible = stats['stock_instances'], stats['num_visible']
     s.cov3D, s.dcov3D = cov3D_precomp, None
     s.splat, s.radii, s.clamped, s.tile_start, s.sorted_ids = splat, radii, clamped, tile_start, sorted_ids
     s.final_T, s.n_contrib, s.image, s.sh = final_T, n_contrib, image, shs is not None
     s.point_count = pc
     s.contrib = contrib
-    s.channels, s.splat_ext, s.log_depth = channels, splat_ext, bool(log_depth)
-    s.num_owners, s.band_ids, s.band_count = num_owners, (band_ids, band_blk, band_rows, band_dsplat), band_count
+    s.splat_ext = splat_ext
+    s.num_owners, s.dsplat = num_owners, band_dsplat
     s.band_counts_host = [int(x) for x in m[_capi.LGR_META_INTS:]] if num_owners > 0 else None
     return image, radii, pid, pwp, pw, s
 
@@ -323,51 +382,29 @@ def rasterize_backward(state: RasterState, grad_image, means3D, opacities, scale
                        peer_stage=None, my_rank=0):
     """Run the backward through the C ABI.  Returns (dmeans3D, dmeans2D, dopacities, dscales, drotations, dcolors, dshs);
     in band mode (state.num_owners > 0) returns the packed gradient rows (M, LGR_ROW_FLOATS) grouped by owner instead."""
-    lib = _capi.load()
     dev = means3D.device
     n = state.n
-    f32 = dict(dtype=torch.float32, device=dev)
     g = _f32c(grad_image, 'grad_image', dev)
-    if state.band_ids[3] is not None:
-        dsplat = state.band_ids[3]          # rows the backward reads were zeroed by the forward's binning kernel
-        state.band_ids = state.band_ids[:3] + (None,)      # one backward per forward
-    else:
-        dsplat = torch.zeros((n, _capi.LGR_GRAD_FLOATS), **f32)
-    if state.num_owners > 0:
-        m_rows = sum(state.band_counts_host)
-        if peer_stage is not None:      # fused exchange: rows are stored straight into the owners' staging buffers
-            _capi.check(lib.lgr_backward(ctypes.byref(state.view), n, state.num_instances, _ptr(means3D), _ptr(opacities),
-                                         _ptr(scales), _ptr(rotations), _ptr(colors_precomp), None, _ptr(state.splat),
-                                         _ptr(state.radii), None, _ptr(state.tile_start), _ptr(state.sorted_ids),
-                                         _ptr(state.image), _ptr(g), _ptr(dsplat), None, None, None, None, None, None, None,
-                                         None, ctypes.c_void_p(peer_stage.data_ptr()), int(my_rank), m_rows, _stream(dev)), 'lgr_backward')
-            return None
-        rows = torch.empty((m_rows, _capi.LGR_ROW_FLOATS), **f32)
-        _capi.check(lib.lgr_backward(ctypes.byref(state.view), n, state.num_instances, _ptr(means3D), _ptr(opacities),
-                                     _ptr(scales), _ptr(rotations), _ptr(colors_precomp), None, _ptr(state.splat),
-                                     _ptr(state.radii), None, _ptr(state.tile_start), _ptr(state.sorted_ids),
-                                     _ptr(state.image), _ptr(g), _ptr(dsplat), None, None, None, None, None, None, None,
-                                     ctypes.c_void_p(rows.data_ptr()) if rows.numel() else _ptr(dsplat), None, 0, m_rows, _stream(dev)),
-                    'lgr_backward')
-        return rows
-    dmeans3D = torch.empty((n, 3), **f32)
-    dmeans2D = torch.empty((n, 3), **f32)
-    dopac = torch.empty((n,), **f32)
-    cov = state.cov3D is not None
-    dscales = None if cov else torch.empty((n, 3), **f32)
-    drot = None if cov else torch.empty((n, 4), **f32)
-    if cov:      # stock cov3D_precomp: the covariance gradient replaces the scale / rotation gradients
-        state.dcov3D = torch.empty((n, 6), **f32)
-        state.view.dcov3D_d = state.dcov3D.data_ptr()
-    dcolors = torch.empty((n, 3 if state.log_depth else state.channels), **f32) if colors_precomp is not None else None
-    dshs = torch.empty((n,) + tuple(shs.shape[1:]), **f32) if shs is not None else None
-    _capi.check(lib.lgr_backward(ctypes.byref(state.view), n, state.num_instances, _ptr(means3D), _ptr(opacities),
-                                 _ptr(scales), _ptr(rotations), _ptr(colors_precomp), _ptr(shs), _ptr(state.splat),
-                                 _ptr(state.radii), _ptr(state.clamped), _ptr(state.tile_start), _ptr(state.sorted_ids),
-                                 _ptr(state.image), _ptr(g), _ptr(dsplat), _ptr(dmeans3D),
-                                 _ptr(dmeans2D), _ptr(dopac), _ptr(dscales), _ptr(drot), _ptr(dcolors), _ptr(dshs), None,
-                                 None, 0, 0, _stream(dev)), 'lgr_backward')
-    return dmeans3D, dmeans2D, dopac, dscales, drot, dcolors, dshs
+    dsplat, state.dsplat = state.dsplat, None      # band mode's rows, zeroed by the forward: one backward per forward
+    if dsplat is None:
+        dsplat = torch.zeros((n, _capi.LGR_GRAD_FLOATS), dtype=torch.float32, device=dev)
+    if state.num_owners == 0:
+        grads, state.dcov3D = backward_per_gaussian(state.view, n, state.num_instances, (means3D, opacities, scales, rotations,
+                                                    colors_precomp, shs), state.splat, state.radii, state.clamped,
+                                                    state.tile_start, state.sorted_ids, state.image, g, dsplat)
+        return grads
+    m_rows = sum(state.band_counts_host)
+    # the rows go to `rows`, or with peer_stage (fused exchange) straight into the owners' staging buffers; with no rows
+    # at all dsplat stands in for the non-NULL grad_rows that selects the rows output
+    rows = None if peer_stage is not None else torch.empty((m_rows, _capi.LGR_ROW_FLOATS), dtype=torch.float32, device=dev)
+    grad_rows = None if rows is None else _ptr(rows) if rows.numel() else _ptr(dsplat)
+    _capi.check(_capi.load().lgr_backward(ctypes.byref(state.view), n, state.num_instances, _ptr(means3D), _ptr(opacities),
+                                          _ptr(scales), _ptr(rotations), _ptr(colors_precomp), None, _ptr(state.splat),
+                                          _ptr(state.radii), None, _ptr(state.tile_start), _ptr(state.sorted_ids),
+                                          _ptr(state.image), _ptr(g), _ptr(dsplat), None, None, None, None, None, None, None,
+                                          grad_rows, _ptr(peer_stage), int(my_rank) if peer_stage is not None else 0, m_rows,
+                                          _stream(dev)), 'lgr_backward')
+    return rows
 
 
 def point_id_count(point_count: torch.Tensor):
@@ -392,8 +429,7 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacities, colors_precomp, shs, scales, rotations, settings, filter_mode, want_aux,
-                tile_rows, raw_params=False, prezero_dsplat=False, instance_capacity=None, holder=None, cov3D_precomp=None,
-                log_depth=False):
+                tile_rows, raw_params=False, instance_capacity=None, holder=None, cov3D_precomp=None, log_depth=False):
         dev = means3D.device
         m = _f32c(means3D, 'means3D')
         o = _f32c(opacities, 'opacities', dev)
@@ -403,9 +439,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         c = _f32c(colors_precomp, 'colors_precomp', dev)
         sh = _f32c(shs, 'shs', dev)
         image, radii, pid, pwp, pw, state = rasterize_forward(settings, m, o, sc, r, c, sh, filter_mode, want_aux, tile_rows,
-                                                              raw_params=raw_params, prezero_dsplat=prezero_dsplat,
-                                                              instance_capacity=instance_capacity, cov3D_precomp=cov,
-                                                              log_depth=log_depth)
+                                                              raw_params=raw_params, instance_capacity=instance_capacity,
+                                                              cov3D_precomp=cov, log_depth=log_depth)
         if holder is not None:
             holder['state'] = state
         state.image = None          # the backward re-reads the rendered image: saved below so autograd guards it
@@ -437,7 +472,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.state.image = None
         if ctx.debug and m.is_cuda:
             torch.cuda.synchronize(m.device)
-        return (dm3, dm2, dop.reshape(ctx.opacity_shape), dcol, dsh, dsc, drot, None, None, None, None, None, None, None, None,
+        return (dm3, dm2, dop.reshape(ctx.opacity_shape), dcol, dsh, dsc, drot, None, None, None, None, None, None, None,
                 ctx.state.dcov3D, None)
 
 
@@ -494,14 +529,10 @@ class GaussianRasterizer(nn.Module):
         if raw_params and shs is not None and colors_precomp is None:
             raise NotImplementedError('raw_params with SH: pass the raw DC colours as colors_precomp and the REST coefficients '
                                       '(LoG layout, activation.py:27-34) as shs')
-        # will a backward follow?  (decided here: inside autograd.Function.forward grad mode is always off)
-        needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in
-                                                     (means3D, means2D, opacities, colors_precomp, shs, scales, rotations, cov3D_precomp))
         holder = {}
         out = _RasterizeGaussians.apply(means3D, means2D, opacities, colors_precomp, shs, scales, rotations,
                                         self.raster_settings, filter_mode, fork, self.tile_rows, raw_params,
-                                        PREZERO_DSPLAT and needs_grad, self.instance_capacity, holder, cov3D_precomp,
-                                        bool(render_depth))
+                                        self.instance_capacity, holder, cov3D_precomp, bool(render_depth))
         self.last_state = holder.get('state')
         if self.raster_settings.debug and means3D.is_cuda:      # stock `debug`: surface a kernel fault at the call that caused it
             torch.cuda.synchronize(means3D.device)

@@ -1,13 +1,25 @@
-"""Tile-sharded multi-GPU rendering (SURVEY.md 8e, BASELINE config 4): one process per GPU, Gaussians replicated,
-each rank renders a contiguous band of 16-pixel tile rows, and the per-Gaussian gradients -- the only exchange step
-of the path -- are reduced to their owner rank (Gaussian index blocks) over NCCL.
+"""Tile-row multi-GPU rendering (SURVEY.md 8e, BASELINE config 4): one process per GPU, each rank renders a contiguous
+band of 16-pixel tile rows (tile_row_partition) and owns a block of Gaussian indices (owner_partition).  Two modes:
+
+  * shard mode (SplatExchange, the default for more than one GPU): each rank holds only the Gaussians it owns, projects
+    them and pushes the visible splat records to the band owners over peer memory; the band owners return the 2D
+    gradients, and each rank runs the per-Gaussian backward of its own Gaussians.  Nothing is replicated or reduced.
+  * band mode (rasterize_forward with num_owners > 0): the Gaussians are replicated, and the per-Gaussian gradient rows
+    of each band go to their owner rank, over NCCL (exchange_rows_to_owners) or straight into the owners' staging
+    buffers over NVLink (PeerExchange).
 
 The reference has no multi-GPU path at all (`cfg.gpus` only sets CUDA_VISIBLE_DEVICES, apps/train.py:136-137).
 """
+import ctypes
+import os
 from typing import List, Tuple
 
 import torch
 import torch.distributed as dist
+
+from . import _capi
+from .rasterizer import (_f32c, _make_view, _ptr, _stream, _view_tiles, backward_per_gaussian, decode_meta, project,
+                         rasterize_backward, render)
 
 GRAD_FLOATS_PRECOMP = 17   # means3D 3 + means2D 3 + opacity 1 + scales 3 + rotations 4 + colors 3
 
@@ -49,8 +61,6 @@ def unpack_grads(buf: torch.Tensor):
 def rows_to_shard(rows: torch.Tensor, lo: int, hi: int, shard: torch.Tensor = None) -> torch.Tensor:
     """Add packed gradient rows (M, LGR_ROW_FLOATS) whose id lies in [lo,hi) into the dense owner shard
     (hi-lo, LGR_ROW_FLOATS); columns 0..16 are the 17 gradient floats in pack_grads order."""
-    import ctypes
-    from . import _capi
     lib = _capi.load()
     if shard is None:
         shard = torch.zeros((max(hi - lo, 0), _capi.LGR_ROW_FLOATS), dtype=torch.float32, device=rows.device)
@@ -105,7 +115,6 @@ class PeerExchange:
 
     def __init__(self, num_gaussians: int, group=None):
         import torch.distributed._symmetric_memory as symm
-        from . import _capi
         self.group = group if group is not None else dist.group.WORLD
         self.world, self.rank = dist.get_world_size(self.group), dist.get_rank(self.group)
         self.n = int(num_gaussians)
@@ -122,9 +131,6 @@ class PeerExchange:
     def backward(self, state, grad_image, means3D, opacities, scales, rotations, colors_precomp) -> torch.Tensor:
         """Blend backward + per-Gaussian backward with rows pushed to the owners; returns this rank's reduced shard
         (owner_chunk, LGR_ROW_FLOATS): [:, :17] gradients in pack_grads order, [:, 18] the radius."""
-        import ctypes
-        from . import _capi
-        from .rasterizer import rasterize_backward
         lib = _capi.load()
         self.handle.barrier()           # every owner has consumed the previous step's rows
         rasterize_backward(state, grad_image, means3D, opacities, scales, rotations, colors_precomp, None,
@@ -140,9 +146,10 @@ class PeerExchange:
 
 # ---------------------------------------------------------------------------------------------------------------------
 # Shard mode: Gaussians sharded over the ranks, splat records pushed to the band owners, 2D gradients returned.
-# (csrc/lgr_shard.cu; C ABI: lgr_shard_send / lgr_shard_recv_bin / lgr_blend_backward / lgr_shard_return_rows /
-# lgr_shard_gather.)  Unlike band mode above nothing is replicated and no per-Gaussian gradient is ever reduced: the rank
-# that owns a Gaussian projects it, and runs its backward, exactly once.
+# (csrc/lgr_shard.cu; C ABI: lgr_shard_send / lgr_shard_recv_bin_aux / lgr_blend_backward / lgr_shard_return_packed /
+# lgr_shard_gather_packed, between rasterizer.py's project, render and backward_per_gaussian stages.)  Unlike band mode
+# above nothing is replicated and no per-Gaussian gradient is ever reduced: the rank that owns a Gaussian projects it,
+# and runs its backward, exactly once.
 # ---------------------------------------------------------------------------------------------------------------------
 def owner_of_row(tile_row: int, image_height: int, world_size: int) -> int:
     """Rank whose band (tile_row_partition) holds `tile_row`; mirrors owner_of_row() in csrc/lgr_shard.cu."""
@@ -161,7 +168,6 @@ def shard_layout(num_gaussians: int, world_size: int, rank: int):
     gradients, optimiser state and all per-step scratch DO shrink with R; only this staging area does not.  The kernels
     touch the count[s] used rows of a region, except the receive-side counting pass, which also walks the unused slots to
     clear their stale radii."""
-    from . import _capi
     cap = owner_chunk(num_gaussians, world_size)
     rows = world_size * cap
     off = 0
@@ -199,7 +205,6 @@ class SplatExchange:
     with plain local buffers and a no-op barrier, phase by phase."""
 
     def __init__(self, num_gaussians: int, image_height: int, rank: int, world: int, own_buffer, peer_ptrs, barrier):
-        from . import _capi
         self.n, self.rank, self.world = int(num_gaussians), int(rank), int(world)
         if not 0 < self.world <= _capi.LGR_SHARD_MAX_RANKS:
             raise ValueError(f'shard mode supports 1..{_capi.LGR_SHARD_MAX_RANKS} ranks, got {world}')
@@ -235,7 +240,6 @@ class SplatExchange:
         # -- no host synchronisation inside a step, so a step can be captured in a CUDA graph.  The caller then owns the
         # check: check_overflow() tells whether a step outgrew its buffers (its outputs are invalid: redo it).  Off by
         # default because a training loop changes the view every step and D with it.
-        import os
         self.sync_free = bool(int(os.environ.get('LGR_SYNC_FREE', '0')))
         self._inst_cap = 0
 
@@ -270,9 +274,6 @@ class SplatExchange:
     def project_and_send(self, settings, means3D, opacities, scales, rotations, colors_precomp=None, shs=None,
                          filter_mode=None, want_aux=True, raw_params=False, render_depth=False) -> ShardStep:
         """Project this rank's shard (inputs are the LOCAL rows [lo,hi) of the model) and push the visible records."""
-        import ctypes
-        from . import _capi
-        from .rasterizer import _f32c, _make_view, _ptr, _stream
         lib = _capi.load()
         if render_depth:
             raise _capi.LgrError('render_depth is not available in shard mode: the exchange moves three-channel records only')
@@ -295,52 +296,35 @@ class SplatExchange:
         # the receive and render kernels visit only the rows the sources filled (the first count[s] of each region)
         s.view_band.region_count_d = self.buf.data_ptr() + 4 * int(self.layout.off_count)
         s.view_band.region_cap, s.view_band.num_regions = self.cap, self.world
-        H, W = s.view_full.image_height, s.view_full.image_width
-        if H != self.image_height:
+        if s.view_full.image_height != self.image_height:
             raise ValueError('image height differs from the one the bands were cut for')
-        gx, gy = (W + 15) // 16, (H + 15) // 16
-        i32 = dict(dtype=torch.int32, device=dev)
-        s.splat = self._scratch('splat', (n, _capi.LGR_SPLAT_FLOATS), torch.float32)
-        s.radii = torch.empty((n,), **i32)                                   # returned to the caller: never recycled
-        s.clamped = self._scratch('clamped', (n,), torch.uint8) if sh is not None else None
-        s.tile_start_full = self._scratch('tile_start_full', (gx * gy + 1,), torch.int32)
-        cursor = self._scratch('cursor_full', (_capi.LGR_TILE_SCRATCH_INTS * gx * gy,), torch.int32)
-        meta = self._scratch('meta_full', (_capi.LGR_META_INTS,), torch.int32)
-        st = _stream()
-        _capi.check(lib.lgr_forward_project(ctypes.byref(s.view_full), n, _ptr(m), _ptr(o), _ptr(sc), _ptr(r), _ptr(c), _ptr(sh),
-                                            _ptr(s.splat), _ptr(s.radii), _ptr(s.clamped), _ptr(s.tile_start_full), _ptr(cursor),
-                                            _ptr(meta), st), 'lgr_forward_project')
+        # radii is returned to the caller; the other buffers are recycled
+        s.splat, s.radii, s.clamped, s.tile_start_full, _, _ = project(s.view_full, n, self._scratch, m, o, sc, r, c, sh)
         s.send_scratch = self._scratch('send', (_capi.shard_send_ints(n, self.world),), torch.int32)
         _capi.check(lib.lgr_shard_send(ctypes.byref(s.view_full), ctypes.byref(self.layout), n, self.lo, _ptr(s.splat),
-                                       _ptr(s.radii), _ptr(s.send_scratch), ctypes.c_void_p(self.peer_ptrs.data_ptr()), st),
+                                       _ptr(s.radii), _ptr(s.send_scratch), ctypes.c_void_p(self.peer_ptrs.data_ptr()), _stream()),
                     'lgr_shard_send')
         return s
 
     def receive_and_render(self, s: ShardStep):
         """Bin, sort and blend the rows received for this rank's band.  Returns (image, radii of the local shard,
         point_id_pixel with GLOBAL Gaussian indices, point_weight_pixel); image / maps are full size, band rows filled."""
-        import ctypes
-        from . import _capi
-        from .rasterizer import _ptr, _stream, set_contrib_lists, use_contrib_lists
         lib = _capi.load()
         dev = self.buf.device
         v = s.view_band
         H, W = v.image_height, v.image_width
-        gx = (W + 15) // 16
-        ntiles = gx * (self.band[1] - self.band[0])
+        ntiles = _view_tiles(v)
         rows = self.world * self.cap
         i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
         s.tile_start = self._scratch('tile_start', (ntiles + 1,), torch.int32)
         cursor = self._scratch('cursor', (_capi.LGR_TILE_SCRATCH_INTS * max(ntiles, 1),), torch.int32)
-        meta = self.meta
-        st = _stream()
         s.pw_rows = s.pc_rows = None
         if s.want_aux:      # per-row aux accumulators of the blend; their used rows are zeroed by the counting kernel
             s.pw_rows = self._scratch('pw_rows', (rows,), torch.float32)
             s.pc_rows = self._scratch('pc_rows', (rows,), torch.int32)
         _capi.check(lib.lgr_shard_recv_bin_aux(ctypes.byref(v), ctypes.byref(self.layout), _ptr(self.buf), _ptr(self.dsplat_rows),
-                                               _ptr(s.tile_start), _ptr(cursor), _ptr(meta), _ptr(s.pw_rows), _ptr(s.pc_rows), st),
-                    'lgr_shard_recv_bin_aux')
+                                               _ptr(s.tile_start), _ptr(cursor), _ptr(self.meta), _ptr(s.pw_rows), _ptr(s.pc_rows),
+                                               _stream()), 'lgr_shard_recv_bin_aux')
         s.image = torch.zeros((3, H, W), **f32)                              # outputs: fresh every step
         final_T = self._scratch('final_T', (H, W), torch.float32)            # written for the band's pixels, read by nobody
         n_contrib = self._scratch('n_contrib', (H, W), torch.int32)
@@ -348,47 +332,27 @@ class SplatExchange:
         if s.want_aux:
             pid = torch.full((H, W), -1, **i32)
             pwp = torch.zeros((H, W), **f32)
+        cap = stats = None
         if self.sync_free and self._inst_cap > 0:
             cap = self._inst_cap
-            inst_key = self._scratch('inst_key', (cap,), torch.int32)
-            inst_val = self._scratch('inst_val', (cap,), torch.int32)
-            inst_tmp = self._scratch('inst_tmp', (2 * cap,), torch.int32)      # the binning's staging buffer
-            s.sorted_ids = self._scratch('sorted_ids', (cap,), torch.int32)
-            set_contrib_lists(v, self._scratch('contrib', (2 * cap + ntiles,), torch.int32) if use_contrib_lists(cap, None) else None,
-                              cap, n_contrib)
             s.num_instances, s.max_tile_len, s.num_rows, s.stock_instances = cap, None, None, None      # see stats()
-            _capi.check(lib.lgr_forward_render_device_sized(ctypes.byref(v), rows, cap, _ptr(meta), _ptr(self.recv_splat), _ptr(self.recv_radii),
-                                                            _ptr(s.tile_start), _ptr(cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp), _ptr(s.sorted_ids),
-                                                            _ptr(s.image), _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp),
-                                                            _ptr(s.pw_rows), _ptr(s.pc_rows), st), 'lgr_forward_render_device_sized')
-            return s.image, s.radii, pid, pwp
-        h = self.header.tolist()                                     # the one host sync of a host-sized forward (160 bytes)
-        m = h[32:40]
-        D, max_len, num_long = int(m[0]), int(m[1]), int(m[5])
-        s.num_instances, s.max_tile_len, s.num_rows = D, max_len, int(sum(h[:self.world]))
-        s.stock_instances = (m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32)
-        if max_len <= lib.lgr_sort_smem_capacity():
-            self._inst_cap = max(self._inst_cap, D + D // 4 + 4096)
-        inst_key = self._scratch('inst_key', (D,), torch.int32)
-        inst_val = self._scratch('inst_val', (D,), torch.int32)
-        inst_tmp = self._scratch('inst_tmp', (2 * D,), torch.int32)      # the binning's staging buffer (and the sort's scratch)
-        s.sorted_ids = self._scratch('sorted_ids', (D,), torch.int32)
-        set_contrib_lists(v, self._scratch('contrib', (2 * D + ntiles,), torch.int32) if use_contrib_lists(D, max_len) else None,
-                          D, n_contrib)
-        _capi.check(lib.lgr_forward_render(ctypes.byref(v), rows, D, max_len, num_long, _ptr(self.recv_splat), _ptr(self.recv_radii),
-                                           _ptr(s.tile_start), _ptr(cursor), _ptr(inst_key), _ptr(inst_val), _ptr(inst_tmp),
-                                           _ptr(s.sorted_ids), _ptr(s.image), _ptr(final_T), _ptr(n_contrib), _ptr(pid), _ptr(pwp),
-                                           _ptr(s.pw_rows), _ptr(s.pc_rows), st), 'lgr_forward_render')
+        else:
+            h = self.header.tolist()                                     # the one host sync of a host-sized forward (160 bytes)
+            stats = decode_meta(h[32:40])
+            s.num_instances, s.max_tile_len, s.stock_instances = stats['num_instances'], stats['max_tile_len'], stats['stock_instances']
+            s.num_rows = int(sum(h[:self.world]))
+            if s.max_tile_len <= lib.lgr_sort_smem_capacity():
+                self._inst_cap = max(self._inst_cap, s.num_instances + s.num_instances // 4 + 4096)
+        s.sorted_ids, _ = render(v, rows, self.recv_splat, self.recv_radii, s.tile_start, cursor, self.meta, s.image, final_T,
+                                 n_contrib, pid, pwp, s.pw_rows, s.pc_rows, self._scratch, cap, stats)
         return s.image, s.radii, pid, pwp
 
     def stats(self):
-        """Counters of the last received step, read back from the exchange header (synchronises): dict with num_rows,
-        num_instances, stock_instances, max_tile_len, overflow (non-zero: a device-sized step outgrew its buffers and its
-        outputs are invalid -- redo it with sync_free = False, which also re-learns the capacity)."""
+        """Counters of the last received step, read back from the exchange header (synchronises): decode_meta()'s dict
+        and num_rows, the rows received.  overflow non-zero: a device-sized step outgrew its buffers and its outputs are
+        invalid -- redo it with sync_free = False, which also re-learns the capacity."""
         h = self.header.tolist()
-        m = h[32:40]
-        return dict(num_rows=int(sum(h[:self.world])), num_instances=int(m[0]), max_tile_len=int(m[1]),
-                    stock_instances=(m[2] & 0xffffffff) | ((m[3] & 0xffffffff) << 32), overflow=int(m[6]))
+        return dict(decode_meta(h[32:40]), num_rows=int(sum(h[:self.world])))
 
     def check_overflow(self):
         """Raise if the last device-sized step did not fit its instance buffers (one 160-byte read-back)."""
@@ -402,9 +366,6 @@ class SplatExchange:
     def blend_backward_and_return(self, s: ShardStep, grad_image):
         """Gradient sweep over this rank's band, then the 2D gradients (and the per-row aux outputs) go back to the ranks
         that pushed the rows."""
-        import ctypes
-        from . import _capi
-        from .rasterizer import _f32c, _ptr, _stream
         lib = _capi.load()
         s.grad_image = _f32c(grad_image, 'grad_image', self.buf.device)
         st, L, peers = _stream(), self.layout, ctypes.c_void_p(self.peer_ptrs.data_ptr())
@@ -419,32 +380,18 @@ class SplatExchange:
         """Sum the returned rows per local Gaussian and run the per-Gaussian backward of the local shard.  Returns
         ((dmeans3D, dmeans2D, dopacities, dscales, drotations, dcolors, dshs), point_weight, point_count) for the
         Gaussians [lo,hi) this rank owns."""
-        import ctypes
-        from . import _capi
-        from .rasterizer import _ptr, _stream
         lib = _capi.load()
         dev = self.buf.device
         n = s.n
-        m, o, sc, r, c, sh = s.inputs
-        f32 = dict(dtype=torch.float32, device=dev)
         dsplat = self._scratch('dsplat_local', (n, _capi.LGR_GRAD_FLOATS), torch.float32)
-        pw = torch.empty((n,), **f32) if s.want_aux else None
+        pw = torch.empty((n,), dtype=torch.float32, device=dev) if s.want_aux else None
         pc = torch.empty((n,), dtype=torch.int32, device=dev) if s.want_aux else None
-        st = _stream()
         _capi.check(lib.lgr_shard_gather_packed(ctypes.byref(s.view_full), ctypes.byref(self.layout), n, _ptr(s.splat), _ptr(s.radii),
-                                                _ptr(s.send_scratch), _ptr(self.buf), _ptr(dsplat), _ptr(pw), _ptr(pc), st),
+                                                _ptr(s.send_scratch), _ptr(self.buf), _ptr(dsplat), _ptr(pw), _ptr(pc), _stream()),
                     'lgr_shard_gather_packed')
-        dmeans3D, dmeans2D = torch.empty((n, 3), **f32), torch.empty((n, 3), **f32)
-        dopac, dscales, drot = torch.empty((n,), **f32), torch.empty((n, 3), **f32), torch.empty((n, 4), **f32)
-        dcolors = torch.empty((n, 3), **f32) if c is not None else None
-        dshs = torch.empty_like(sh) if sh is not None else None
-        if n:
-            _capi.check(lib.lgr_backward(ctypes.byref(s.view_full), n, 0, _ptr(m), _ptr(o), _ptr(sc), _ptr(r), _ptr(c), _ptr(sh),
-                                         _ptr(s.splat), _ptr(s.radii), _ptr(s.clamped), _ptr(s.tile_start_full), None,
-                                         _ptr(s.image), _ptr(s.grad_image), _ptr(dsplat), _ptr(dmeans3D), _ptr(dmeans2D),
-                                         _ptr(dopac), _ptr(dscales), _ptr(drot), _ptr(dcolors), _ptr(dshs), None, None, 0, 0, st),
-                        'lgr_backward')
-        return (dmeans3D, dmeans2D, dopac, dscales, drot, dcolors, dshs), pw, pc
+        grads, _ = backward_per_gaussian(s.view_full, n, 0, s.inputs, s.splat, s.radii, s.clamped, s.tile_start_full, None,
+                                         s.image, s.grad_image, dsplat)
+        return grads, pw, pc
 
     # ---- the calls a training loop makes -----------------------------------------------------------------------
     def forward(self, settings, means3D, opacities, scales, rotations, colors_precomp=None, shs=None, **kw):

@@ -40,9 +40,7 @@ def main():
     *_, st = rasterize_forward(settings, d['means3D'], d['opacities'].reshape(-1), d['scales'], d['rotations'],
                                d['colors'] if deg == 0 else None, d['shs'] if deg > 0 else None, LGR_FILTER_MAX, True)
     torch.cuda.synchronize()
-    lists = next(t for t in st.keep if t is not None and t.data_ptr() == st.view.contrib_id_d)
-    D = st.num_instances
-    count = lists[2 * D:].cpu().numpy().astype(np.int64)
+    count = st.contrib_lists()[2].cpu().numpy().astype(np.int64)
     start = st.tile_start.cpu().numpy().astype(np.int64)
     nc = st.n_contrib.cpu().numpy()
     gx, gy = (W + 15) // 16, (H + 15) // 16
