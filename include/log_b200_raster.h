@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 25
+#define LGR_ABI_VERSION 26
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -539,6 +539,41 @@ int lgr_photometric_backward(int32_t batch, int32_t channels, int32_t height, in
 int lgr_corrector_step(int64_t num_views, int64_t index, int32_t start_step, double log_lr_init, double log_lr_final,
                        int32_t* steps_d, float* param_d, float* grad_d, float* exp_avg_d, float* exp_avg_sq_d,
                        float* max_exp_avg_sq_d, void* stream);
+
+/* LoG's densification rebuild (Splitter.split_and_remove / split_and_remove_other, LoG/model/splitter.py:138-220): every
+ * table of P rows becomes [rows with ~remove, in index order] ++ [N rows per split parent, parents in ascending index],
+ * remove = flag_remove | flag_split when remove_split is set.  Four calls, one host read between the first two:
+ *   lgr_densify_plan      split_d, remove_d: (P) bool flags.  result_d (LGR_DENSIFY_RESULTS int64) receives num_keep, S
+ *                         (split parents) and the count of remove_d; scratch_d: LGR_DENSIFY_SCRATCH_INTS(P) int32, kept
+ *                         until lgr_densify_map.  P < 2^31.
+ *   lgr_densify_map       map_d (num_keep + S) int64: the kept rows, then the split parents.
+ *   lgr_densify_children  N in {2, 4, 8}: children_d (2 N S, 3) fp32 receives the children's xyz (N S rows, parent-major),
+ *                         then their raw scaling (split_by_uniform, splitter.py:5-31 and 95-130, in LoG's fp32 rounding),
+ *                         from the parents map_d + num_keep of the raw tables xyz_d (P,3), scaling_d (P,3) and
+ *                         rotation_d (P,4); result_d's doubles at LGR_DENSIFY_STATS the four means split_by_uniform
+ *                         prints (parent scale, parent max scale, child scale, child max scale).  partial_d:
+ *                         LGR_DENSIFY_PARTIAL_DOUBLES doubles.
+ *   lgr_densify_gather    dst_d (num_keep + N S rows of row_bytes) from src_d (P rows): row r < num_keep copies
+ *                         src[map[r]]; appended row j takes, by mode, the parent src[map[num_keep + j / N]]
+ *                         (LGR_DENSIFY_REPEAT), appended_d row j (LGR_DENSIFY_CHILDREN) or zeros (LGR_DENSIFY_ZERO). */
+#define LGR_DENSIFY_RESULTS 8
+#define LGR_DENSIFY_KEEP 0
+#define LGR_DENSIFY_SPLIT 1
+#define LGR_DENSIFY_REMOVED 2
+#define LGR_DENSIFY_STATS 4          /* four doubles in the int64 slots 4..7 */
+#define LGR_DENSIFY_REPEAT 0
+#define LGR_DENSIFY_CHILDREN 1
+#define LGR_DENSIFY_ZERO 2
+#define LGR_DENSIFY_SCRATCH_INTS(P) (2 * (((int64_t)(P) + 255) / 256) + 2 + ((int64_t)(P) + 3) / 4)
+#define LGR_DENSIFY_PARTIAL_DOUBLES 2112
+int lgr_densify_plan(int64_t num_rows, const uint8_t* split_d, const uint8_t* remove_d, int32_t remove_split,
+                     int32_t* scratch_d, int64_t* result_d, void* stream);
+int lgr_densify_map(int64_t num_rows, int64_t num_keep, const int32_t* scratch_d, int64_t* map_d, void* stream);
+int lgr_densify_children(int64_t num_keep, int64_t num_split, int32_t n, const int64_t* map_d, const float* xyz_d,
+                         const float* scaling_d, const float* rotation_d, float* children_d, double* partial_d,
+                         int64_t* result_d, void* stream);
+int lgr_densify_gather(int64_t num_keep, int64_t num_split, int32_t n, int64_t row_bytes, int32_t mode, const int64_t* map_d,
+                       const void* src_d, const void* appended_d, void* dst_d, void* stream);
 
 /* Depth-supervision loss (LoG's NaiveRendererAndLoss.append_depth_loss, renderer.py:268-292, with MiDaS's
  * ScaleAndShiftInvariantLoss(alpha=0.5, scales=1), LoG/render/loss.py:47-117).  For each of the 64 patches k, the 64x64

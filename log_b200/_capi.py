@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 25
+LGR_ABI_VERSION = 26
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -23,7 +23,8 @@ EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'l
            'lgr_shard_gather', 'lgr_shard_recv_bin_aux', 'lgr_shard_return_packed', 'lgr_shard_gather_packed', 'lgr_tree_traverse', 'lgr_mark_visible',
            'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis',
            'lgr_counter_update', 'lgr_log_step', 'lgr_prepare_cull', 'lgr_prepare_select', 'lgr_photometric_forward',
-           'lgr_photometric_backward', 'lgr_corrector_step')
+           'lgr_photometric_backward', 'lgr_corrector_step', 'lgr_densify_plan', 'lgr_densify_map', 'lgr_densify_children',
+           'lgr_densify_gather')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -129,6 +130,17 @@ class LgrStep(ctypes.Structure):
                 ('radius3d_min_d', _vp), ('radius3d_max_d', _vp)]
 
 
+LGR_DENSIFY_RESULTS = 8
+LGR_DENSIFY_KEEP, LGR_DENSIFY_SPLIT, LGR_DENSIFY_REMOVED, LGR_DENSIFY_STATS = 0, 1, 2, 4
+LGR_DENSIFY_REPEAT, LGR_DENSIFY_CHILDREN, LGR_DENSIFY_ZERO = 0, 1, 2
+LGR_DENSIFY_PARTIAL_DOUBLES = 2112
+
+
+def densify_scratch_ints(num_rows):
+    """LGR_DENSIFY_SCRATCH_INTS."""
+    return 2 * ((num_rows + 255) // 256) + 2 + (num_rows + 3) // 4
+
+
 class LgrError(RuntimeError):
     pass
 
@@ -207,6 +219,14 @@ def bind(lib):
                                                                                               _vp, _vp]
     lib.lgr_log_step.restype = ctypes.c_int
     lib.lgr_log_step.argtypes = [ctypes.POINTER(LgrStep), _i64, _i64, _vp, _vp, _vp, _vp]
+    lib.lgr_densify_plan.restype = ctypes.c_int
+    lib.lgr_densify_plan.argtypes = [_i64, _vp, _vp, _i32, _vp, _vp, _vp]
+    lib.lgr_densify_map.restype = ctypes.c_int
+    lib.lgr_densify_map.argtypes = [_i64, _i64, _vp, _vp, _vp]
+    lib.lgr_densify_children.restype = ctypes.c_int
+    lib.lgr_densify_children.argtypes = [_i64, _i64, _i32] + [_vp] * 8
+    lib.lgr_densify_gather.restype = ctypes.c_int
+    lib.lgr_densify_gather.argtypes = [_i64, _i64, _i32, _i64, _i32] + [_vp] * 5
     lib.lgr_profile_enable.restype = ctypes.c_int
     lib.lgr_profile_enable.argtypes = [ctypes.c_int]
     lib.lgr_profile_collect.restype = ctypes.c_int

@@ -58,6 +58,11 @@ int launch_depth_loss_bwd(int, int, int, int, const float*, const int64_t*, cons
                           const int64_t*, const int64_t*, const int64_t*, const double*, float*, const float*, float*,
                           cudaStream_t);
 int launch_depth_vis(int, int, const float*, const int64_t*, const float*, const int64_t*, float*, float*, cudaStream_t);
+int launch_densify_plan(int64_t, const uint8_t*, const uint8_t*, int, int32_t*, int64_t*, cudaStream_t);
+int launch_densify_map(int64_t, int64_t, const int32_t*, int64_t*, cudaStream_t);
+int launch_densify_children(int64_t, int, const int64_t*, const float*, const float*, const float*, float*, double*, int64_t*,
+                            cudaStream_t);
+int launch_densify_gather(int64_t, int64_t, int, int64_t, int, const int64_t*, const void*, const void*, void*, cudaStream_t);
 }  // namespace lgr
 
 using namespace lgr;
@@ -604,6 +609,41 @@ int lgr_prepare_select(const lgr_prepare* prep, const lgr_tree* tree, const floa
   a.fx = focal_x; a.fy = focal_y; a.tanfovx = tan_fovx; a.tanfovy = tan_fovy; a.min_px = min_resolution_pixel;
   const int levels = tree->max_level < max_depth ? tree->max_level : max_depth;
   return launch_prepare_select(*prep, a, tree->num_nodes, levels, point_weight_d, meta_d, (cudaStream_t)stream);
+}
+
+/* ---- LoG's densification rebuild ---- */
+static bool split_n_ok(int32_t n) { return n == 2 || n == 4 || n == 8; }
+
+int lgr_densify_plan(int64_t num_rows, const uint8_t* split_d, const uint8_t* remove_d, int32_t remove_split,
+                     int32_t* scratch_d, int64_t* result_d, void* stream) {
+  if (num_rows < 0 || !result_d || (num_rows > 0 && (!split_d || !remove_d || !scratch_d))) return LGR_E_BADARG;
+  if (num_rows > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  return launch_densify_plan(num_rows, split_d, remove_d, remove_split ? 1 : 0, scratch_d, result_d, (cudaStream_t)stream);
+}
+
+int lgr_densify_map(int64_t num_rows, int64_t num_keep, const int32_t* scratch_d, int64_t* map_d, void* stream) {
+  if (num_rows < 0 || num_keep < 0 || num_keep > num_rows || (num_rows > 0 && (!scratch_d || !map_d))) return LGR_E_BADARG;
+  if (num_rows > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  return launch_densify_map(num_rows, num_keep, scratch_d, map_d, (cudaStream_t)stream);
+}
+
+int lgr_densify_children(int64_t num_keep, int64_t num_split, int32_t n, const int64_t* map_d, const float* xyz_d,
+                         const float* scaling_d, const float* rotation_d, float* children_d, double* partial_d,
+                         int64_t* result_d, void* stream) {
+  if (num_keep < 0 || num_split < 0 || !split_n_ok(n)) return LGR_E_BADARG;
+  if (num_split > 0 && (!map_d || !xyz_d || !scaling_d || !rotation_d || !children_d || !partial_d || !result_d)) return LGR_E_BADARG;
+  return launch_densify_children(num_split, n, map_d + num_keep, xyz_d, scaling_d, rotation_d, children_d, partial_d, result_d,
+                                 (cudaStream_t)stream);
+}
+
+int lgr_densify_gather(int64_t num_keep, int64_t num_split, int32_t n, int64_t row_bytes, int32_t mode, const int64_t* map_d,
+                       const void* src_d, const void* appended_d, void* dst_d, void* stream) {
+  if (num_keep < 0 || num_split < 0 || !split_n_ok(n) || row_bytes <= 0) return LGR_E_BADARG;
+  if (mode != LGR_DENSIFY_REPEAT && mode != LGR_DENSIFY_CHILDREN && mode != LGR_DENSIFY_ZERO) return LGR_E_BADARG;
+  const int64_t rows_out = num_keep + n * num_split;
+  if (rows_out > 0 && (!map_d || !src_d || !dst_d)) return LGR_E_BADARG;
+  if (mode == LGR_DENSIFY_CHILDREN && num_split > 0 && !appended_d) return LGR_E_BADARG;
+  return launch_densify_gather(num_keep, rows_out, n, row_bytes, mode, map_d, src_d, appended_d, dst_d, (cudaStream_t)stream);
 }
 
 /* ---- diagnostics: per-kernel CUDA-event timing (used by bench.py for the live roofline numbers) ---- */
