@@ -1,8 +1,8 @@
 /* log_b200_raster.h -- C ABI of the H100-native differentiable Gaussian-splatting rasteriser.
  *
  * This is the drop-in boundary for the hot path of zju3dv/LoG.  Plain pointers and sizes only; no torch types.
- * All pointers named *_d are DEVICE pointers (fp32 / int32, contiguous, 16-byte aligned); `stream` is a
- * cudaStream_t passed as void*.  Every function returns 0 on success, a positive cudaError_t value if the CUDA
+ * All pointers named *_d are DEVICE pointers (fp32 / int32, contiguous, 16-byte aligned) unless an entry point says
+ * otherwise; `stream` is a cudaStream_t passed as void*.  Every function returns 0 on success, a positive cudaError_t value if the CUDA
  * runtime reported one, or a negative LGR_E_* code.  Nothing here ever falls back to the CPU.
  *
  * What each entry point replaces in the reference (paths relative to a zju3dv/LoG checkout):
@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 26
+#define LGR_ABI_VERSION 27
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -413,7 +413,8 @@ int lgr_point_compact(int64_t n, const int32_t* point_count_d, int32_t* scratch_
  * i = index_d[k]:   m = b1 m + (1-b1) g ;  v = b2 v + (1-b2) g^2 ;  [vmax = max(vmax, v)] ;
  *                   param -= lr / (1 - b1^step) * m / (sqrt(v or vmax) / sqrt(1 - b2^step) + eps)
  * in place on param_d / exp_avg_d / exp_avg_sq_d [/ max_exp_avg_sq_d, NULL = no amsgrad] (N, row_floats);
- * grad_d is the compact (rows, row_floats) gradient of the gathered rows; index_d int64 (rows), unique. */
+ * grad_d is the compact (rows, row_floats) gradient of the gathered rows; index_d int64 (rows), unique.
+ * exp_avg_d, exp_avg_sq_d and max_exp_avg_sq_d may be mapped page-locked host memory (LGR_HOST_STATE). */
 int lgr_sparse_adam(int64_t rows, int32_t row_floats, const int64_t* index_d, const float* grad_d, float* param_d,
                     float* exp_avg_d, float* exp_avg_sq_d, float* max_exp_avg_sq_d, int64_t step, double lr, double beta1,
                     double beta2, double eps, void* stream);
@@ -445,6 +446,14 @@ int lgr_counter_update(const lgr_counter* counter, int64_t num_leaf, int64_t num
                        const int64_t* grad_strides, int64_t num_points, const void* point_id_d, const void* point_count_d,
                        int32_t id_bytes, int32_t count_bytes, uint8_t* flag_vis_d, void* stream);
 
+/* LGR_HOST_STATE: the optimiser moments (exp_avg_d, exp_avg_sq_d, max_exp_avg_sq_d of lgr_sparse_adam and lgr_step_key)
+ * and the tables src_d / dst_d of lgr_densify_gather may each be device memory or page-locked host memory mapped into
+ * the device's address space (cudaHostAlloc / cudaHostRegister; cudaPointerGetAttributes type cudaMemoryTypeHost with a
+ * device pointer equal to the host pointer), which the kernels read and write over the host link.  Every other pointer
+ * must be device memory of one device.  The entry points check every non-NULL pointer on the host before they enqueue
+ * anything, also for 0 rows, and return LGR_E_BADARG for pageable host memory, another device's memory, managed memory
+ * or host memory where device memory is required. */
+
 /* One key of LoG.step (level_of_gaussian.py:379-398): the parameter table getattr(gaussian, key) and its optimiser state,
  * all (N, row_floats) float32 contiguous, and the compact (rows, row_floats) gradient of the gathered rows. */
 #define LGR_STEP_MAX_KEYS 8
@@ -467,13 +476,25 @@ typedef struct lgr_step {
   float beta1, beta2, one_minus_beta1, one_minus_beta2, eps;
   const float* radius3d_min_d; /* (N) Counter.radius3d_min / radius3d_max, read by the clamp */
   const float* radius3d_max_d;
+  const int64_t* order_d;      /* NULL: rows in their own order; else lgr_step_order's list, visited in its order */
 } lgr_step;
 /* SparseOptimizer.step + LoG.clamp_scale for rows r < num_leaf + num_node with flag_vis_d[r] (uint8), on Gaussian g(r)
  * as in lgr_counter_update: per key with a gradient the update of lgr_sparse_adam on row g(r) with grad_d[r], then for
  * the clamp key min(max(s, logf(radius3d_min[g])), logf(radius3d_max[g])) (NaN propagates, as torch.clamp).  Rows
- * without flag_vis are not touched.  The g(r) of flagged rows must be unique.  One launch for every key. */
+ * without flag_vis are not touched.  The g(r) of flagged rows must be unique.  One launch for every key.  The moments
+ * may be host-resident (LGR_HOST_STATE); with order_d the threads visit the rows order_d lists instead of r, so that
+ * neighbouring threads touch neighbouring rows of host tables.  The result is the same bit for bit either way. */
 int lgr_log_step(const lgr_step* step, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
                  const int64_t* index_node_d, const uint8_t* flag_vis_d, void* stream);
+/* The flagged rows of an lgr_log_step call in ascending Gaussian index, without a sort: order_d (num_leaf + num_node)
+ * int64 receives the rows r with flag_vis_d[r] ordered by g(r), then -1 up to its end.  The g(r) of flagged rows must be
+ * unique and below num_gaussians (rows with g(r) >= num_gaussians are left out).  scratch_d:
+ * LGR_STEP_ORDER_SCRATCH_INTS(num_gaussians) int32 (a byte flag and the row of every Gaussian, per-chunk counts).
+ * num_gaussians and num_leaf + num_node < 2^31. */
+#define LGR_STEP_ORDER_SCRATCH_INTS(n) (2 + 2 * (((int64_t)(n) + 255) / 256) + 2 + (int64_t)(n) + ((int64_t)(n) + 3) / 4)
+int lgr_step_order(int64_t num_gaussians, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
+                   const int64_t* index_node_d, const uint8_t* flag_vis_d, int32_t* scratch_d, int64_t* order_d,
+                   void* stream);
 
 /* SSIM loss (LoG's training loss term, renderer.py:253-266): replaces LoG/render/loss.py:6-44 SSIM(11, C)(img1, img2)
  * with reduce=True, i.e. 1 - mean(S) over the valid (B, C, H-10, W-10) map of
@@ -555,7 +576,8 @@ int lgr_corrector_step(int64_t num_views, int64_t index, int32_t start_step, dou
  *                         LGR_DENSIFY_PARTIAL_DOUBLES doubles.
  *   lgr_densify_gather    dst_d (num_keep + N S rows of row_bytes) from src_d (P rows): row r < num_keep copies
  *                         src[map[r]]; appended row j takes, by mode, the parent src[map[num_keep + j / N]]
- *                         (LGR_DENSIFY_REPEAT), appended_d row j (LGR_DENSIFY_CHILDREN) or zeros (LGR_DENSIFY_ZERO). */
+ *                         (LGR_DENSIFY_REPEAT), appended_d row j (LGR_DENSIFY_CHILDREN) or zeros (LGR_DENSIFY_ZERO).
+ *                         src_d and dst_d may be host-resident (LGR_HOST_STATE); map_d and appended_d are device memory. */
 #define LGR_DENSIFY_RESULTS 8
 #define LGR_DENSIFY_KEEP 0
 #define LGR_DENSIFY_SPLIT 1

@@ -12,7 +12,7 @@ LGR_SPLAT_FLOATS = 12
 LGR_GRAD_FLOATS = 12
 LGR_META_INTS = 8
 LGR_TILE_SCRATCH_INTS = 33
-LGR_ABI_VERSION = 26
+LGR_ABI_VERSION = 27
 LGR_CONTRIB_MAX_LIST = 1 << 24
 LGR_STAGE_HEADER_FLOATS = 64
 LGR_ROW_FLOATS = 20
@@ -24,7 +24,7 @@ EXPORTS = ('lgr_abi_version', 'lgr_sort_smem_capacity', 'lgr_compute_radius', 'l
            'lgr_ssim_forward', 'lgr_ssim_backward', 'lgr_depth_loss_forward', 'lgr_depth_loss_backward', 'lgr_depth_vis',
            'lgr_counter_update', 'lgr_log_step', 'lgr_prepare_cull', 'lgr_prepare_select', 'lgr_photometric_forward',
            'lgr_photometric_backward', 'lgr_corrector_step', 'lgr_densify_plan', 'lgr_densify_map', 'lgr_densify_children',
-           'lgr_densify_gather')
+           'lgr_densify_gather', 'lgr_step_order')
 LGR_SHARD_MAX_RANKS = 32
 LGR_PROFILE_KERNELS = 12
 
@@ -127,7 +127,12 @@ class LgrStep(ctypes.Structure):
     """struct lgr_step: the key table of lgr_log_step."""
     _fields_ = [('keys', LgrStepKey * LGR_STEP_MAX_KEYS), ('num_keys', _i32), ('row_floats', _i32), ('beta1', _f32),
                 ('beta2', _f32), ('one_minus_beta1', _f32), ('one_minus_beta2', _f32), ('eps', _f32),
-                ('radius3d_min_d', _vp), ('radius3d_max_d', _vp)]
+                ('radius3d_min_d', _vp), ('radius3d_max_d', _vp), ('order_d', _vp)]
+
+
+def step_order_scratch_ints(num_gaussians):
+    """LGR_STEP_ORDER_SCRATCH_INTS."""
+    return 2 + 2 * ((num_gaussians + 255) // 256) + 2 + num_gaussians + (num_gaussians + 3) // 4
 
 
 LGR_DENSIFY_RESULTS = 8
@@ -219,6 +224,8 @@ def bind(lib):
                                                                                               _vp, _vp]
     lib.lgr_log_step.restype = ctypes.c_int
     lib.lgr_log_step.argtypes = [ctypes.POINTER(LgrStep), _i64, _i64, _vp, _vp, _vp, _vp]
+    lib.lgr_step_order.restype = ctypes.c_int
+    lib.lgr_step_order.argtypes = [_i64, _i64, _i64] + [_vp] * 6
     lib.lgr_densify_plan.restype = ctypes.c_int
     lib.lgr_densify_plan.argtypes = [_i64, _vp, _vp, _i32, _vp, _vp, _vp]
     lib.lgr_densify_map.restype = ctypes.c_int

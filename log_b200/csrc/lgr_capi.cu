@@ -27,6 +27,7 @@ int launch_sparse_adam(int64_t, int, const int64_t*, const float*, float*, float
 int launch_counter_update(const lgr_counter&, int64_t, int64_t, const int64_t*, const int64_t*, const int32_t*, const float*,
                           const float*, const int64_t*, int64_t, const void*, const void*, int, int, uint8_t*, cudaStream_t);
 int launch_log_step(const lgr_step&, int64_t, int64_t, const int64_t*, const int64_t*, const uint8_t*, cudaStream_t);
+int launch_step_order(int64_t, int64_t, int64_t, const int64_t*, const int64_t*, const uint8_t*, int32_t*, int64_t*, cudaStream_t);
 int launch_point_compact(int64_t, const int32_t*, int32_t*, int32_t*, int32_t*, int32_t*, cudaStream_t);
 int launch_blend_bwd(const View&, const int32_t*, const int32_t*, const float*, const float*, const float*, float*,
                      cudaStream_t);
@@ -107,6 +108,37 @@ static int colour_source(const lgr_view* v, int64_t n, const float* colors_preco
   *c = log_sh ? Colour::LOG_SH : shs_d ? Colour::SH : six_precomp ? Colour::RGB6 : Colour::RGB;
   return 0;
 }
+
+// Where the pointers of one call live (LGR_HOST_STATE in the header): device-only pointers must be device memory, state
+// pointers device memory or mapped page-locked host memory, and every device pointer of the call on one device.  A
+// kernel that dereferenced pageable memory would fault the device, so this is checked on the host before any launch.
+// NULL pointers are left to the callers' own checks.  A host compiler of this file (the CPU emulation of the kernels,
+// whose buffers are all host memory the emulated kernels read directly) has no CUDA runtime to ask and checks nothing.
+struct Residence {
+  int device = -1;
+  bool ok = true;
+#ifndef __CUDACC__
+  void need(const void*, bool) {}
+#else
+  void need(const void* p, bool host_ok) {
+    if (!p || !ok) return;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+      (void)cudaGetLastError();      // not a pointer the runtime knows: clear the error it reported
+      ok = false;
+      return;
+    }
+    if (a.type == cudaMemoryTypeDevice) {
+      if (device >= 0 && a.device != device) ok = false;
+      device = a.device;
+      return;
+    }
+    ok = host_ok && a.type == cudaMemoryTypeHost && a.devicePointer == p;
+  }
+#endif
+  void on_device(const void* p) { need(p, false); }
+  void state(const void* p) { need(p, true); }
+};
 
 extern "C" {
 
@@ -259,6 +291,10 @@ int lgr_sparse_adam(int64_t rows, int32_t row_floats, const int64_t* index_d, co
                     double beta2, double eps, void* stream) {
   if (rows < 0 || row_floats <= 0 || step < 1) return LGR_E_BADARG;
   if (rows > 0 && (!index_d || !grad_d || !param_d || !exp_avg_d || !exp_avg_sq_d)) return LGR_E_BADARG;
+  Residence where;
+  where.on_device(param_d); where.on_device(index_d); where.on_device(grad_d);
+  where.state(exp_avg_d); where.state(exp_avg_sq_d); where.state(max_exp_avg_sq_d);
+  if (!where.ok) return LGR_E_BADARG;
   // scalar preparation in double, exactly like the Python reference (sparse_optimizer.py:64-70)
   const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
   const double step_size = lr / bc1;
@@ -292,15 +328,36 @@ int lgr_log_step(const lgr_step* step, int64_t num_leaf, int64_t num_node, const
   if ((num_leaf > 0 && !index_leaf_d) || (num_node > 0 && !index_node_d) || (num_leaf + num_node > 0 && !flag_vis_d))
     return LGR_E_BADARG;
   int32_t prefix = 0;
+  Residence where;
   for (int k = 0; k < step->num_keys; k++) {      // the keys tile a row in order
     const lgr_step_key& key = step->keys[k];
     if (key.row_floats <= 0 || key.prefix != prefix || !key.param_d) return LGR_E_BADARG;
     if (key.grad_d && (!key.exp_avg_d || !key.exp_avg_sq_d)) return LGR_E_BADARG;
     if (key.clamp && (key.row_floats != 3 || !step->radius3d_min_d || !step->radius3d_max_d)) return LGR_E_BADARG;
     prefix += key.row_floats;
+    where.on_device(key.param_d); where.on_device(key.grad_d);
+    where.state(key.exp_avg_d); where.state(key.exp_avg_sq_d); where.state(key.max_exp_avg_sq_d);
   }
   if (prefix != step->row_floats) return LGR_E_BADARG;
+  where.on_device(step->radius3d_min_d); where.on_device(step->radius3d_max_d); where.on_device(step->order_d);
+  where.on_device(index_leaf_d); where.on_device(index_node_d); where.on_device(flag_vis_d);
+  if (!where.ok) return LGR_E_BADARG;
   return launch_log_step(*step, num_leaf, num_node, index_leaf_d, index_node_d, flag_vis_d, (cudaStream_t)stream);
+}
+
+int lgr_step_order(int64_t num_gaussians, int64_t num_leaf, int64_t num_node, const int64_t* index_leaf_d,
+                   const int64_t* index_node_d, const uint8_t* flag_vis_d, int32_t* scratch_d, int64_t* order_d,
+                   void* stream) {
+  if (num_gaussians < 0 || num_leaf < 0 || num_node < 0) return LGR_E_BADARG;
+  if ((num_leaf > 0 && !index_leaf_d) || (num_node > 0 && !index_node_d)) return LGR_E_BADARG;
+  if (num_leaf + num_node > 0 && (!flag_vis_d || !order_d || (num_gaussians > 0 && !scratch_d))) return LGR_E_BADARG;
+  if (num_gaussians > 0x7fffffffLL || num_leaf + num_node > 0x7fffffffLL) return LGR_E_UNSUPPORTED;
+  Residence where;
+  where.on_device(index_leaf_d); where.on_device(index_node_d); where.on_device(flag_vis_d);
+  where.on_device(scratch_d); where.on_device(order_d);
+  if (!where.ok) return LGR_E_BADARG;
+  return launch_step_order(num_gaussians, num_leaf, num_node, index_leaf_d, index_node_d, flag_vis_d, scratch_d, order_d,
+                           (cudaStream_t)stream);
 }
 
 // Shape, pointers and strides of an lgr_ssim_* call; the grid (one CTA per 32x32 tile of every plane) must fit one dimension.
@@ -643,6 +700,9 @@ int lgr_densify_gather(int64_t num_keep, int64_t num_split, int32_t n, int64_t r
   const int64_t rows_out = num_keep + n * num_split;
   if (rows_out > 0 && (!map_d || !src_d || !dst_d)) return LGR_E_BADARG;
   if (mode == LGR_DENSIFY_CHILDREN && num_split > 0 && !appended_d) return LGR_E_BADARG;
+  Residence where;
+  where.on_device(map_d); where.on_device(appended_d); where.state(src_d); where.state(dst_d);
+  if (!where.ok) return LGR_E_BADARG;
   return launch_densify_gather(num_keep, rows_out, n, row_bytes, mode, map_d, src_d, appended_d, dst_d, (cudaStream_t)stream);
 }
 

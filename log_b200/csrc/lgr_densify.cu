@@ -28,7 +28,7 @@ constexpr int DENS_GRID = LGR_TREE_GRID;
 static_assert(4 * DENS_GRID <= LGR_DENSIFY_PARTIAL_DOUBLES, "one partial per CTA and statistic");
 
 int launch_compact_scan(int64_t, int32_t*, int64_t*, int64_t*, cudaStream_t);
-int launch_compact_scatter(int64_t, const uint8_t*, const int32_t*, int64_t*, int64_t*, cudaStream_t);
+int launch_compact_scatter(int64_t, const uint8_t*, const int32_t*, const int32_t*, int64_t*, int64_t*, cudaStream_t);
 
 // bits[row]: bit 0 = kept, bit 1 = split parent; two counts per chunk; result[LGR_DENSIFY_REMOVED] += flag_remove rows
 __global__ void __launch_bounds__(DENS_THREADS)
@@ -180,7 +180,7 @@ int launch_densify_plan(int64_t P, const uint8_t* split, const uint8_t* remove, 
 int launch_densify_map(int64_t P, int64_t num_keep, const int32_t* scratch, int64_t* map, cudaStream_t st) {
   if (P == 0) return 0;
   const uint8_t* bits = reinterpret_cast<const uint8_t*>(scratch + 2 * ((P + DENS_THREADS - 1) / DENS_THREADS) + 2);
-  return launch_compact_scatter(P, bits, scratch, map, map + num_keep, st);
+  return launch_compact_scatter(P, bits, scratch, nullptr, map, map + num_keep, st);
 }
 
 int launch_densify_children(int64_t S, int N, const int64_t* parents, const float* xyz, const float* scaling,

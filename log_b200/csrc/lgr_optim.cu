@@ -8,7 +8,12 @@
 //   counter_update_kernel  Counter.update_by_output (LoG/model/counter.py:36-68) for one view: one thread per rendered
 //                          row, then one per point_id entry; plain read-modify-writes on unique rows
 //   log_step_kernel        LoG.step (level_of_gaussian.py:379-398): every key's Adam update and the scale clamp
-//                          (:367-377), one thread per (row, float) across all keys
+//                          (:367-377), one thread per (row, float) across all keys; rows in their own order, or in the
+//                          order step_order builds
+//   step_order             the flagged rows in ascending Gaussian index for moments held in host memory (read over the
+//                          host link, where a row's few bytes per table cost a request each and neighbouring rows share
+//                          requests and TLB entries): one byte flag and the row per Gaussian, then lgr_prepare.cu's
+//                          order-preserving compaction over the Gaussians -- no sort
 //   corrector_step_kernel  Corrector.step (LoG/model/corrector.py:35-62) for one view: one warp, the step count, LoG's
 //                          skip before start_step and its learning-rate schedule on the device
 #include "lgr_common.cuh"
@@ -157,9 +162,10 @@ log_step_kernel(const __grid_constant__ lgr_step s, int64_t num_leaf, int64_t to
                 const int64_t* __restrict__ node, const uint8_t* __restrict__ flag_vis) {
   const int64_t t = (int64_t)blockIdx.x * ADAM_THREADS + threadIdx.x;
   if (t >= total) return;
-  const int64_t r = t / s.row_floats;
-  if (!flag_vis[r]) return;
-  int col = (int)(t - r * s.row_floats), k = 0;
+  const int64_t i = t / s.row_floats;
+  const int64_t r = s.order_d ? s.order_d[i] : i;
+  if (r < 0 || !flag_vis[r]) return;
+  int col = (int)(t - i * s.row_floats), k = 0;
   while (k + 1 < s.num_keys && col >= s.keys[k + 1].prefix) k++;
   const lgr_step_key& key = s.keys[k];
   col -= key.prefix;
@@ -182,6 +188,62 @@ int launch_log_step(const lgr_step& s, int64_t num_leaf, int64_t num_node, const
                                                                                                  node, flag_vis);
   LGR_CHECK_LAUNCH();
   return 0;
+}
+
+// ---- the ordered pass: flagged rows in ascending Gaussian index ------------------------------------------------------
+
+constexpr int ORDER_THREADS = COMPACT_CHUNK;
+#ifndef LGR_TREE_GRID
+#define LGR_TREE_GRID 528               // 4 CTAs per SM on the 132 SMs of an H100 SXM; grid-stride loops cover any size
+#endif
+
+int launch_compact_scan(int64_t, int32_t*, int64_t*, int64_t*, cudaStream_t);
+int launch_compact_scatter(int64_t, const uint8_t*, const int32_t*, const int32_t*, int64_t*, int64_t*, cudaStream_t);
+
+// bits[g] = 1 and row_of[g] = r for every flagged row r (bits zeroed before)
+__global__ void __launch_bounds__(ORDER_THREADS)
+step_mark_kernel(int64_t rows, int64_t num_leaf, const int64_t* __restrict__ leaf, const int64_t* __restrict__ node,
+                 const uint8_t* __restrict__ flag_vis, int64_t n, uint8_t* __restrict__ bits, int32_t* __restrict__ row_of) {
+  for (int64_t r = (int64_t)blockIdx.x * ORDER_THREADS + threadIdx.x; r < rows; r += (int64_t)gridDim.x * ORDER_THREADS) {
+    if (!flag_vis[r]) continue;
+    const int64_t g = row_gaussian(r, num_leaf, leaf, node);
+    if ((uint64_t)g >= (uint64_t)n) continue;
+    bits[g] = 1;
+    row_of[g] = (int32_t)r;
+  }
+}
+
+// the flagged Gaussians of each chunk, as the (A, B) pairs lgr_prepare.cu's scan takes (B empty)
+__global__ void __launch_bounds__(ORDER_THREADS)
+step_count_kernel(int64_t n, const uint8_t* __restrict__ bits, int32_t* __restrict__ chunk_cnt) {
+  const int64_t nchunks = (n + ORDER_THREADS - 1) / ORDER_THREADS;
+  for (int64_t chunk = blockIdx.x; chunk < nchunks; chunk += gridDim.x) {
+    const int64_t g = chunk * ORDER_THREADS + threadIdx.x;
+    const int c = __syncthreads_count(g < n && bits[g]);
+    if (threadIdx.x == 0) { chunk_cnt[2 * chunk] = c; chunk_cnt[2 * chunk + 1] = 0; }
+  }
+}
+
+// scratch layout (int32 units): count [2, one int64] | chunk counts [2 ceil(n/256) + 2] | row_of [n] | bits [n bytes]
+int launch_step_order(int64_t n, int64_t num_leaf, int64_t num_node, const int64_t* leaf, const int64_t* node,
+                      const uint8_t* flag_vis, int32_t* scratch, int64_t* order, cudaStream_t st) {
+  const int64_t rows = num_leaf + num_node;
+  if (rows == 0) return 0;
+  cudaError_t e = cudaMemsetAsync(order, 0xff, sizeof(int64_t) * (size_t)rows, st);      // -1 past the count
+  if (e != cudaSuccess || n == 0) return (int)e;
+  int64_t* count = reinterpret_cast<int64_t*>(scratch);
+  int32_t* chunk_cnt = scratch + 2;
+  int32_t* row_of = chunk_cnt + 2 * ((n + ORDER_THREADS - 1) / ORDER_THREADS) + 2;
+  uint8_t* bits = reinterpret_cast<uint8_t*>(row_of + n);
+  e = cudaMemsetAsync(bits, 0, (size_t)n, st);
+  if (e != cudaSuccess) return (int)e;
+  step_mark_kernel<<<LGR_TREE_GRID, ORDER_THREADS, 0, st>>>(rows, num_leaf, leaf, node, flag_vis, n, bits, row_of);
+  LGR_CHECK_LAUNCH();
+  step_count_kernel<<<LGR_TREE_GRID, ORDER_THREADS, 0, st>>>(n, bits, chunk_cnt);
+  LGR_CHECK_LAUNCH();
+  const int rc = launch_compact_scan(n, chunk_cnt, count, nullptr, st);
+  if (rc) return rc;
+  return launch_compact_scatter(n, bits, chunk_cnt, row_of, order, nullptr, st);
 }
 
 // ---- Corrector.step: one row of the (V, 3) view-correction table ----------------------------------------------------

@@ -143,8 +143,9 @@ prep_scan_kernel(int64_t n_host, const int64_t* __restrict__ n_d, int32_t* __res
 // stable compaction: A-slots to out_a, B-slots to out_b, each in slot order; a slot contributes cand[slot], or the slot
 // itself when cand is null.  pad_a: out_a[total_a .. n) = -1 (the gather list of the visibility render, whose rows past
 // the count are empty)
+template <class Cand>
 __global__ void __launch_bounds__(PREP_THREADS)
-prep_scatter_kernel(int64_t n_host, const int64_t* __restrict__ n_d, const int64_t* __restrict__ cand,
+prep_scatter_kernel(int64_t n_host, const int64_t* __restrict__ n_d, const Cand* __restrict__ cand,
                     const uint8_t* __restrict__ bits, const int32_t* __restrict__ chunk_pre, int64_t* __restrict__ out_a,
                     int64_t* __restrict__ out_b, const int64_t* __restrict__ total_a, int pad_a) {
   __shared__ __align__(16) int wa[PREP_THREADS / 32];
@@ -161,8 +162,8 @@ prep_scatter_kernel(int64_t n_host, const int64_t* __restrict__ n_d, const int64
     int pa = chunk_pre[2 * chunk], pb = chunk_pre[2 * chunk + 1];
     for (int w = 0; w < wid; w++) { pa += wa[w]; pb += wb[w]; }
     const unsigned lt = (1u << lane) - 1u;
-    if (f & 1) out_a[pa + __popc(ba & lt)] = cand ? cand[slot] : slot;
-    if (f & 2) out_b[pb + __popc(bb & lt)] = cand ? cand[slot] : slot;
+    if (f & 1) out_a[pa + __popc(ba & lt)] = cand ? (int64_t)cand[slot] : slot;
+    if (f & 2) out_b[pb + __popc(bb & lt)] = cand ? (int64_t)cand[slot] : slot;
     __syncthreads();
   }
   if (pad_a) {
@@ -201,23 +202,24 @@ static int prep_compact(const PrepArgs& a, const PrepScratch& s, int64_t n_host,
   LGR_CHECK_LAUNCH();
   prep_scan_kernel<<<1, 1024, 0, st>>>(n_host, n_d, s.chunk_cnt, total_a, total_b);
   LGR_CHECK_LAUNCH();
-  prep_scatter_kernel<<<PREP_GRID, PREP_THREADS, 0, st>>>(n_host, n_d, s.cand, s.bits, s.chunk_cnt, out_a, out_b, total_a,
-                                                        pad_a ? 1 : 0);
+  prep_scatter_kernel<int64_t><<<PREP_GRID, PREP_THREADS, 0, st>>>(n_host, n_d, s.cand, s.bits, s.chunk_cnt, out_a, out_b,
+                                                                 total_a, pad_a ? 1 : 0);
   LGR_CHECK_LAUNCH();
   return 0;
 }
 
-// The scan and the scatter of a compaction whose classify pass lives in another file (lgr_densify.cu): bits and chunk
-// counts as prep_classify_kernel writes them, chunks of COMPACT_CHUNK slots, and the slot ids as the output.
+// The scan and the scatter of a compaction whose classify pass lives in another file (lgr_densify.cu, lgr_optim.cu): bits
+// and chunk counts as prep_classify_kernel writes them, chunks of COMPACT_CHUNK slots, and as the output cand[slot], or
+// the slot ids when cand is null.
 int launch_compact_scan(int64_t n, int32_t* chunk_cnt, int64_t* total_a, int64_t* total_b, cudaStream_t st) {
   prep_scan_kernel<<<1, 1024, 0, st>>>(n, nullptr, chunk_cnt, total_a, total_b);
   LGR_CHECK_LAUNCH();
   return 0;
 }
 
-int launch_compact_scatter(int64_t n, const uint8_t* bits, const int32_t* chunk_pre, int64_t* out_a, int64_t* out_b,
-                           cudaStream_t st) {
-  prep_scatter_kernel<<<PREP_GRID, PREP_THREADS, 0, st>>>(n, nullptr, nullptr, bits, chunk_pre, out_a, out_b, nullptr, 0);
+int launch_compact_scatter(int64_t n, const uint8_t* bits, const int32_t* chunk_pre, const int32_t* cand, int64_t* out_a,
+                           int64_t* out_b, cudaStream_t st) {
+  prep_scatter_kernel<int32_t><<<PREP_GRID, PREP_THREADS, 0, st>>>(n, nullptr, cand, bits, chunk_pre, out_a, out_b, nullptr, 0);
   LGR_CHECK_LAUNCH();
   return 0;
 }

@@ -9,6 +9,7 @@ import torch
 from . import _capi
 from ._capi import (LGR_DENSIFY_CHILDREN, LGR_DENSIFY_KEEP, LGR_DENSIFY_PARTIAL_DOUBLES, LGR_DENSIFY_REPEAT,
                     LGR_DENSIFY_RESULTS, LGR_DENSIFY_STATS, LGR_DENSIFY_ZERO, densify_scratch_ints)
+from .optim import host_state
 from .rasterizer import _ptr
 
 _DTYPES = (torch.float32, torch.int32, torch.int16, torch.int8)
@@ -23,13 +24,31 @@ def _flags(flag_split, flag_remove, rows, device):
     return flag_split.contiguous(), flag_remove.contiguous()
 
 
-def _check_table(t, name, rows, device, dim=None):
-    if t.device != device:
-        raise ValueError(f'{name} is on {t.device}, the tables on {device}: tables held elsewhere (the CPU offload of the '
-                         'optimiser state) are not supported')
+def _check_table(t, name, rows, device, dim=None, state=False):
+    """A table of `rows` rows on `device`; with `state`, an optimiser-state table, which may also be host-resident
+    (log_b200.optim.host_state: on the CPU while the tables are on a CUDA device, used page-locked)."""
+    if t.device != device and not (state and t.device.type == 'cpu' and device.type == 'cuda'):
+        raise ValueError(f'{name} is on {t.device}, the tables on {device}: only optimiser state may be held elsewhere, and '
+                         'only on the CPU (LoG\'s offload) while the tables are on a CUDA device')
     if t.dtype not in _DTYPES or not t.is_contiguous() or t.dim() == 0 or t.shape[0] != rows or (dim and t.dim() != dim):
         raise ValueError(f'{name} must be a contiguous float32 / int32 / int16 / int8 tensor of {rows} rows, got {t.dtype} '
                          f'{tuple(t.shape)}{"" if t.is_contiguous() else " (not contiguous)"}')
+    if state:
+        host_state(t, name, device)
+
+
+def _offload(state):
+    """LoG's `state.to(torch.device('cpu'))` (splitter.py:198-204) as device-to-host copies into page-locked memory, on
+    the current stream: every buffer of the BufferDict (or dict) is replaced by its host copy, as `.to` replaces it."""
+    for key, t in list(state.items()):
+        if t.device.type == 'cpu':
+            continue
+        host = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
+        host.copy_(t, non_blocking=True)
+        if isinstance(state, dict):
+            state[key] = host
+        else:
+            setattr(state, key, host)
 
 
 class _Plan:
@@ -40,6 +59,7 @@ class _Plan:
         lib = _capi.load()
         rows = int(flag_split.shape[0])
         self.n, self.device, self.stream = n, device, _capi.current_stream(device)
+        self.held = []                        # replaced host-resident tables, until the stream has passed the gathers
         self.result = torch.zeros(LGR_DENSIFY_RESULTS, dtype=torch.int64, device=device)
         scratch = torch.empty(densify_scratch_ints(rows), dtype=torch.int32, device=device)
         _capi.check(lib.lgr_densify_plan(rows, _ptr(flag_split), _ptr(flag_remove), int(bool(remove_split)), _ptr(scratch),
@@ -53,13 +73,25 @@ class _Plan:
         return self.num_keep + self.n * self.num_split
 
     def rebuild(self, t, mode, appended=None):
-        """Rebuild table `t` in place (`set_`): kept rows, then per split parent N rows by `mode`."""
-        new = torch.empty((self.rows_out,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+        """Rebuild table `t` in place (`set_`): kept rows, then per split parent N rows by `mode`.  A host-resident table
+        is rebuilt into page-locked memory; the old one is held (`release`), since the pinned pool would hand it out
+        again while the gather may still read it."""
+        host = t.device != self.device
+        new = torch.empty((self.rows_out,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device, pin_memory=host)
         row_bytes = t[0].numel() * t.element_size()
         _capi.check(_capi.load().lgr_densify_gather(self.num_keep, self.num_split, self.n, row_bytes, mode, _ptr(self.map),
                                                     _ptr(t), _ptr(appended), _ptr(new), self.stream), 'lgr_densify_gather')
+        if host:
+            self.held.append(t.untyped_storage())
         with torch.no_grad():
             t.set_(new)
+
+    def release(self, synchronised):
+        """Let the replaced host-resident tables go, once the stream has passed their gathers: after a host read the
+        caller made (`synchronised`), or after a synchronisation of its own."""
+        if self.held and not synchronised:
+            torch.cuda.current_stream(self.device).synchronize()
+        self.held = []
 
 
 def _check_splitter(self):
@@ -78,15 +110,20 @@ def splitter_split_and_remove(self, model, optimizer, flag_split, flag_remove, r
     then N rows per split parent: for `xyz` and `scaling` the children of split_by_uniform (splitter.py:95-130) in
     LoG's fp32 rounding, for the other keys the parent's row repeated.  Each table of `optimizer.state_keys` becomes its
     kept rows, then zeros.  Prints LoG's messages and returns num_keep as a 0-d int64 tensor on the flags' device.  As in
-    LoG, above 50 M rows `exp_avg_sq` and above 100 M rows `exp_avg` move to the CPU after the rebuild.
+    LoG, above 50 M rows `exp_avg_sq` and above 100 M rows `exp_avg` move to the CPU after the rebuild: here by
+    device-to-host copies into page-locked memory, each buffer replaced as LoG's `BufferDict.to` replaces it.
 
     Each table is rebuilt by one `lgr_densify_gather` launch and swapped in with `set_`, so every table -- parameters
-    and optimiser state -- keeps its identity (LoG replaces the state tensors).  Two small host reads per call: the
-    counts before the tables are allocated, and the statistics LoG prints.
+    and optimiser state -- keeps its identity (LoG replaces the state tensors).  Optimiser state on the CPU (offloaded
+    earlier) is rebuilt where it is, into page-locked memory, by the same kernel over the host link (a pageable table is
+    pinned once, in place, first).  Two small host reads per call: the counts before the tables are allocated, and the
+    statistics LoG prints; without split parents, and with host-resident state, a stream synchronisation takes the
+    second one's place, so that the replaced host tables are released only after their gathers.  The tables offloaded
+    at the threshold are filled on the stream: host code that reads them must synchronise it first.
     Raises NotImplementedError for `split_method` other than 'uniform', N not in {2, 4, 8}, a `tree_depth` key, keyword
     arguments for split_by_uniform, or a scaling activation other than 'exp'; ValueError for flags that are not (P,)
     bool on the tables' device, tables that are not contiguous float32 / int32 / int16 / int8 of P rows, or optimiser
-    state on another device (the CPU offload); LgrError for CPU tensors."""
+    state anywhere but on the tables' device or (with the tables on a CUDA device) the CPU; LgrError for CPU tensors."""
     _check_splitter(self)
     if kwargs:
         raise NotImplementedError(f'split_by_uniform keyword arguments {sorted(kwargs)} are not supported')
@@ -112,7 +149,7 @@ def splitter_split_and_remove(self, model, optimizer, flag_split, flag_remove, r
     if optimizer is not None:
         for state_key in optimizer.state_keys:
             for key, t in getattr(optimizer, state_key).items():
-                _check_table(t, f'{state_key}[{key!r}]', rows, device)
+                _check_table(t, f'{state_key}[{key!r}]', rows, device, state=True)
                 states.append(t)
     N = self.N
     plan = _Plan(flag_split, flag_remove, remove_split, N, device)
@@ -138,16 +175,17 @@ def splitter_split_and_remove(self, model, optimizer, flag_split, flag_remove, r
         name = model.__class__.__name__
         print(f'[{name}] split : {S} -> {N * S}')
         print(f'[{name}] radius: {m0:.4f} -> {m2:.4f}, {m1:.4f} -> {m3:.4f}')
+    plan.release(synchronised=S > 0)
     num_keep = plan.result[LGR_DENSIFY_KEEP].clone()
     if optimizer is None:
         return num_keep
     total = int(model.xyz.shape[0])
     if total > _OFFLOAD_ROWS and optimizer.exp_avg.device != torch.device('cpu'):
         print(f'[{self.__class__.__name__}] num points {total} > {_OFFLOAD_ROWS}, move exp_avg_sq to CPU')
-        optimizer.exp_avg_sq.to(torch.device('cpu'))
+        _offload(optimizer.exp_avg_sq)
     if total > _OFFLOAD_ROWS * 2:
         print(f'[{self.__class__.__name__}] num points {total} > {_OFFLOAD_ROWS * 2}, move exp_avg to CPU')
-        optimizer.exp_avg.to(torch.device('cpu'))
+        _offload(optimizer.exp_avg)
     return num_keep
 
 

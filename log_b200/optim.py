@@ -18,15 +18,41 @@ from . import _capi
 from .rasterizer import _ptr
 
 
+def host_state(t, name, device):
+    """Where optimiser-state table `t` may live while the parameters are on `device`: on `device`, or -- with the
+    parameters on a CUDA device -- on the CPU, where LoG's Splitter offloads it (LoG/model/splitter.py:198-204).  A CPU
+    table that is not page-locked is moved into page-locked memory once, in place (a copy, then `set_`, so the tensor
+    keeps its identity and its values); the kernels then read and write it over the host link.  -> True for a
+    host-resident table.  Raises ValueError for any other device."""
+    if t.device == device:
+        return False
+    if t.device.type != 'cpu' or device.type != 'cuda':
+        raise ValueError(f'{name} is on {t.device}, the parameters on {device}: optimiser state must be on the parameters\' '
+                         'device, or offloaded to the CPU while they are on a CUDA device')
+    if not t.is_pinned():
+        pinned = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
+        pinned.copy_(t)
+        with torch.no_grad():
+            t.set_(pinned)
+    return True
+
+
 def sparse_adam_step_(param, grad, exp_avg, exp_avg_sq, index, step, lr, max_exp_avg_sq=None, beta1=0.9, beta2=0.999,
                       eps=1e-15):
-    """In place.  param / exp_avg / exp_avg_sq [/ max_exp_avg_sq]: (N, ...) float32 CUDA, contiguous;
-    index: (K,) int64 unique rows; grad: (K, ...) gradient of the gathered rows param[index]."""
+    """In place.  param / exp_avg / exp_avg_sq [/ max_exp_avg_sq]: (N, ...) float32 contiguous, param on a CUDA device;
+    index: (K,) int64 unique rows; grad: (K, ...) gradient of the gathered rows param[index].  The moments may be on the
+    CPU (LoG's offload), where they are used page-locked (`host_state`)."""
     lib = _capi.load()
-    for name, t in (('param', param), ('grad', grad), ('exp_avg', exp_avg), ('exp_avg_sq', exp_avg_sq)):
-        _capi.require_cuda(t, name)
+    for name, t in (('param', param), ('grad', grad), ('exp_avg', exp_avg), ('exp_avg_sq', exp_avg_sq),
+                    ('max_exp_avg_sq', max_exp_avg_sq)):
+        if t is None:
+            continue
+        if name in ('param', 'grad'):
+            _capi.require_cuda(t, name)
         if t.dtype != torch.float32 or not t.is_contiguous():
             raise TypeError(f'{name} must be contiguous float32')
+        if name not in ('param', 'grad'):
+            host_state(t, name, param.device)
     if index.dtype != torch.int64 or not index.is_contiguous():
         raise TypeError('index must be contiguous int64')
     k = int(index.shape[0])
@@ -128,11 +154,20 @@ def _global_steps(optimizer):
 
 def _table(t, name, device):
     if t.device != device:
-        raise ValueError(f'{name} is on {t.device}, the parameters on {device}: optimiser state held elsewhere (the CPU '
-                         'offload of SparseOptimizer.index_select_optimizer) is not supported')
+        raise ValueError(f'{name} is on {t.device}, the parameters on {device}: it must be on the parameters\' device (only '
+                         'the optimiser moments may be offloaded to the CPU)')
     if t.dtype != torch.float32 or not t.is_contiguous():
         raise ValueError(f'{name} must be a contiguous float32 tensor')
     return _ptr(t)
+
+
+def _state_table(t, name, device):
+    """-> (pointer, host-resident) of an optimiser moment: contiguous float32, on the parameters' device or offloaded
+    (`host_state`)."""
+    if t.dtype != torch.float32 or not t.is_contiguous():
+        raise ValueError(f'{name} must be a contiguous float32 tensor')
+    hosted = host_state(t, name, device)
+    return _ptr(t), hosted
 
 
 def log_step(self):
@@ -149,10 +184,17 @@ def log_step(self):
     `base_iter` it calls `self.view_correction.step()` as LoG does; bind `corrector_step` there (below) so that this
     call, too, runs on the device without a host read.
 
+    Offloaded state: above 50 M Gaussians LoG moves `exp_avg_sq`, above 100 M `exp_avg` too, to the CPU.  Such tables are
+    used in page-locked host memory, read and written by the same kernel over the host link (`host_state`: a pageable
+    table is pinned once, in place); the flagged rows are then visited in ascending Gaussian index (one `lgr_step_order`
+    call before the step).  The results are bit for bit those of the on-device step.
+
     Synchronisation: `optimizer.global_steps` is read once, on the first call (and again only if something else changed
-    it since, e.g. `load_state_dict`); afterwards the step never reads the device.  The Gaussians of the flagged rows
-    must be unique, as LoG's leaves and nodes are.  Raises ValueError for optimiser state on another device than the
-    parameters (the CPU offload branch), non-float32 or non-contiguous parameter / state tables, and
+    it since, e.g. `load_state_dict`); afterwards the step never reads the device, also with offloaded state.  So host
+    code that reads offloaded tables -- `torch.save(model.state_dict())` included -- must synchronise the stream first;
+    LoG's trainer does, with `loss.item()` after every step.  The Gaussians of the flagged rows must be unique, as LoG's
+    leaves and nodes are.  Raises ValueError for optimiser state anywhere but on the parameters' device or (with the
+    parameters on a CUDA device) the CPU, non-float32 or non-contiguous parameter / state tables, and
     NotImplementedError for a scaling activation other than 'exp'."""
     gaussian, opt = self.gaussian, self.optimizer
     act = getattr(gaussian, 'activation', None)
@@ -176,7 +218,7 @@ def log_step(self):
     step = _global_steps(opt)
     beta1, beta2, eps = 0.9, 0.999, 1e-15                      # _single_tensor_adam's defaults, eps as step() passes it
     bc1, bc2_sqrt = 1 - beta1 ** int(step), math.sqrt(1 - beta2 ** int(step))
-    table, keep, prefix = [], [], 0
+    table, keep, prefix, hosted = [], [], 0, False
     keys = [k for k, p in params.items() if p.grad is not None]
     if 'scaling' not in keys:
         keys.append('scaling')
@@ -199,11 +241,12 @@ def log_step(self):
                                  f'{tuple(grad.shape)}')
             grad = grad.contiguous()
             keep.append(grad)
-            entry.update(exp_avg_d=_table(opt.exp_avg[key], f'exp_avg[{key!r}]', device),
-                         exp_avg_sq_d=_table(opt.exp_avg_sq[key], f'exp_avg_sq[{key!r}]', device),
-                         max_exp_avg_sq_d=(_table(opt.max_exp_avg_sq[key], f'max_exp_avg_sq[{key!r}]', device)
-                                           if getattr(opt, 'use_amsgrad', False) else None),
-                         grad_d=_ptr(grad), neg_step_size=-(lr / bc1), bc2_sqrt=bc2_sqrt)
+            states = [(n, getattr(opt, n)[key]) for n in ('exp_avg', 'exp_avg_sq', 'max_exp_avg_sq')
+                      if n != 'max_exp_avg_sq' or getattr(opt, 'use_amsgrad', False)]
+            for n, t in states:
+                entry[n + '_d'], on_host = _state_table(t, f'{n}[{key!r}]', device)
+                hosted = hosted or on_host
+            entry.update(grad_d=_ptr(grad), neg_step_size=-(lr / bc1), bc2_sqrt=bc2_sqrt)
         table.append(_capi.LgrStepKey(**entry))
         prefix += row
     if len(table) > _capi.LGR_STEP_MAX_KEYS:
@@ -211,12 +254,21 @@ def log_step(self):
     counter = self.counter
     for name in ('radius3d_min', 'radius3d_max'):
         _table(getattr(counter, name), f'counter.{name}', device)
+    lib, stream = _capi.load(), _capi.current_stream(device)
+    order = None
+    if hosted:
+        # moments in host memory: visit the flagged rows in ascending Gaussian index (DESIGN.md §3; measured in §4)
+        n = int(scaling.shape[0])
+        scratch = torch.empty(_capi.step_order_scratch_ints(n), dtype=torch.int32, device=device)
+        order = torch.empty(rows, dtype=torch.int64, device=device)
+        _capi.check(lib.lgr_step_order(n, n_leaf, n_node, _ptr(leaf), _ptr(node), _ptr(flag_vis), _ptr(scratch), _ptr(order),
+                                       stream), 'lgr_step_order')
     args = _capi.LgrStep(num_keys=len(table), row_floats=prefix, beta1=beta1, beta2=beta2, one_minus_beta1=1.0 - beta1,
                          one_minus_beta2=1.0 - beta2, eps=eps, radius3d_min_d=_ptr(counter.radius3d_min),
-                         radius3d_max_d=_ptr(counter.radius3d_max))
+                         radius3d_max_d=_ptr(counter.radius3d_max), order_d=_ptr(order))
     args.keys[:len(table)] = table
-    _capi.check(_capi.load().lgr_log_step(ctypes.byref(args), n_leaf, n_node, _ptr(leaf), _ptr(node), _ptr(flag_vis),
-                                          _capi.current_stream(device)), 'lgr_log_step')
+    _capi.check(lib.lgr_log_step(ctypes.byref(args), n_leaf, n_node, _ptr(leaf), _ptr(node), _ptr(flag_vis),
+                                          stream), 'lgr_log_step')
     self.lr = opt.xyz_lr
     if step == self.base_iter:
         print(f'[{self.__class__.__name__}] base iteration {self.base_iter} done, enable view_correction module')
