@@ -8,8 +8,9 @@
 // splats this skips ~90 % of the (pixel, splat) pairs the classic per-thread loop evaluates.
 // Backward: the same front-to-back walk (closed form of the published recurrence, see below).  Per contributing hit every
 // lane publishes two scalars; every 8 hits the warp contracts them against fixed per-pixel weights (pixel-coordinate
-// moments and cotangent-weighted sums) on the tensor cores (mma.sync m16n8k8, split TF32 = fp32 accuracy); the moments
-// become gradients once per staged splat, then 3 vector atomics per splat.  With View::contrib_* the forward writes, per
+// moments and cotangent-weighted sums) on the tensor cores (mma.sync m16n8k8, split TF32 = fp32 accuracy); a warp meets a
+// staged splat at most once, so the contraction holds the warp's whole share of each hit, and one lane per hit turns it
+// into gradients and adds them to dsplat with 3 vector atomics.  With View::contrib_* the forward writes, per
 // tile, the compacted list of the entries some sub-tile composited (with those sub-tiles and the list index), and the
 // backward (REC) stages only that list and walks exactly those pairs, stopping every pixel after its last contributor (the
 // forward's n_contrib) instead of re-testing boxes and transmittances.
@@ -98,9 +99,6 @@ __device__ __forceinline__ uint32_t pin_reg(uint32_t v) {
 }
 __device__ __forceinline__ void red_shared_max_u32(uint32_t addr, unsigned v) {
   asm volatile("red.shared.max.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void red_shared_add_f32(uint32_t addr, float v) {
-  asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
 }
 __device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
@@ -363,22 +361,25 @@ blend_fwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
 // on the tensor cores: A (16 rows = 8 wG rows + 8 w rows) straight from the blocks with ldmatrix, B = the weights (moment
 // weights are small half-integers and their products: exact in TF32; the cotangent weights are split hi + lo once per
 // kernel), every A value split hi + lo, fp32 accumulation -- 8 + 12 mma.m16n8k8 per 8 hits, error ~2^-20 relative.
-// The D fragments (hit x output) are added into per-splat shared accumulators.  The moments are turned
-// into d/dmean2D, d/dconic, d/dopacity once per staged splat when the batch is flushed (X = splat centre, same
-// coordinates):
+// A splat appears once in a tile's list, so the D fragments (hit x output) hold the warp's whole contribution to each of
+// its pending hits: lane (g, 0) gathers hit g's outputs from lanes (g, 1..2) with shuffles, turns the moments into
+// d/dmean2D, d/dconic, d/dopacity (X = splat centre, same coordinates)
 //     sum wG dx = X M00 - M10,   sum wG dx^2 = X^2 M00 - 2 X M10 + M20,   sum wG dx dy = XY M00 - X M01 - Y M10 + M11 ...
+// and adds them to dsplat with 3 vector atomics: no shared accumulators, no shared-memory float atomics (a CAS loop in
+// SASS), no flush between the batch barriers.  The sums are linear in the moments, so the warps' shares add up in dsplat
+// to what one transform of the tile's summed moments gives, up to rounding.
 constexpr int HITS = 8;          // hits per contraction (half the m of mma.m16n8k8: 8 wG rows + 8 w rows)
 constexpr int XROW = 36;         // floats per published row: 32 pixels + 4 pad, so the 8 rows of an ldmatrix block hit 8 bank groups
-constexpr int BWD_SMEM = BATCH * 48 + BATCH * 36 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 192 + 192) * 4 + BATCH;
-// six channels: 64-byte records, 12 accumulators per splat, a cotangent table of 6 columns (65 792 bytes)
-constexpr int BWD6_SMEM = BATCH * 64 + BATCH * 48 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 384 + 192) * 4 + BATCH;
+constexpr int BWD_SMEM = BATCH * 48 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 192 + 192) * 4 + BATCH;
+// six channels: 64-byte records, a cotangent table of 6 columns (53 504 bytes)
+constexpr int BWD6_SMEM = BATCH * 64 + (BLEND_THREADS / 32) * (2 * HITS * XROW + 384 + 192) * 4 + BATCH;
 
 // REC: the forward wrote the compacted list of the entries that some sub-tile composited, with those sub-tiles and the
 // entry's list index (View::contrib_*), and (View::last_contrib = its n_contrib output) where every pixel's last
 // contributor sits; the sweep stages only that list, meets exactly the contributing (sub-tile, splat) pairs, and a pixel
 // is finished once the walk has passed its last contributor -- no box tests, no T < 1e-4 test.
 // SIX: six colour channels.  R_j and c . dL/dC run over the six; the cotangent B operand fills 6 of the 8 columns (same mma
-// count); 12 accumulators per splat (moments, then the six colour sums), flushed with three float4 atomics.
+// count); the six colour sums go out with the third float4 atomic.
 template <bool REC, bool SIX = false>
 __global__ void __launch_bounds__(BLEND_THREADS, SIX ? LGR_BWD6_MIN_CTAS : LGR_BWD_MIN_CTAS)
 blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* __restrict__ sorted_ids,
@@ -387,12 +388,10 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   constexpr int F4 = SIX ? 4 : 3;                // float4 per staged record
   constexpr uint32_t RB = 16u * F4;             // its stride in bytes
   constexpr int NCH = SIX ? 6 : 3;              // colour channels = used columns of the cotangent B operand
-  constexpr int NG = 6 + NCH;                   // accumulators per staged splat: 6 moments + the colour sums
   constexpr int NCW = 64 * NCH;                 // floats of a warp's cotangent table: 4 k-steps x NCH*4 lanes x 4
   extern __shared__ float4 smem_f4[];
   float4* s_rec = smem_f4;                                                        // [BATCH * F4]
-  float* s_g = reinterpret_cast<float*>(s_rec + BATCH * F4);                      // [BATCH * NG]
-  float* s_x = s_g + BATCH * NG;                                                  // per warp: wG[8][36] | w[8][36]
+  float* s_x = reinterpret_cast<float*>(s_rec + BATCH * F4);                      // per warp: wG[8][36] | w[8][36]
   float* s_cw = s_x + (BLEND_THREADS / 32) * 2 * HITS * XROW;                     // per warp: cotangent weights, hi/lo, A-fragment order
   float* s_mw = s_cw + (BLEND_THREADS / 32) * NCW;                                // per warp: moment weights, A-fragment order
   unsigned char* s_bits = reinterpret_cast<unsigned char*>(s_mw + (BLEND_THREADS / 32) * 192);      // [BATCH]
@@ -401,14 +400,12 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   const float pxf = (float)st.x, pyf = (float)st.y;
   const float tx0 = (float)((tile % v.gx) * TILE), ty0 = (float)((v.row0 + tile / v.gx) * TILE);
   const int beg = tile_start[tile], len = tile_start[tile + 1] - beg;
-  const uint32_t s_g_addr = pin_reg(smem_u32(s_g));
   const uint32_t s_rec_addr = pin_reg(smem_u32(s_rec));
   const uint32_t xg_addr = pin_reg(smem_u32(s_x) + (uint32_t)warp * (2 * HITS * XROW * 4));
   const uint32_t xlane_addr = pin_reg(xg_addr + 4u * (uint32_t)lane);
   // ldmatrix row address of this lane: row lane%8 of block lane/8; blocks = (wG, chunk 2s), (w, chunk 2s), (wG, chunk 2s+1), (w, chunk 2s+1)
   const uint32_t xrow = pin_reg(xg_addr + (uint32_t)(lane & 7) * (XROW * 4) + (uint32_t)((lane >> 3) & 1) * (HITS * XROW * 4) +
                                 (uint32_t)(lane >> 4) * 16u);
-  const float tcx = tx0 + 7.5f, tcy = ty0 + 7.5f;
   const int g = lane >> 2, t = lane & 3;        // mma fragment coordinates of this lane
 
   float Rd = 0.f, dp0 = 0.f, dp1 = 0.f, dp2 = 0.f;
@@ -459,16 +456,13 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
   int id_next = tid < len ? ids[beg + tid] : -1;
   if (tid >= n) id_next = -1;
 
-  // Two barriers per batch, as in the forward: thread tid stages, flushes and re-stages only slot tid (record, hit bits and
-  // the nine accumulators of that splat).
+  // Two barriers per batch, as in the forward: thread tid stages and re-stages only slot tid (record and hit bits).
   int base = 0, cnt = min(BATCH, n);
   auto stage = [&]() {
     if (tid < cnt) {
       // REC: walk exactly the (sub-tile, splat) pairs that composited something in the forward
       stage_splat<SIX>(s_rec, s_bits, tid, splat, id_next, tx0, ty0, REC ? v.contrib_entry + beg + base + tid : nullptr,
                        v.splat_ext);
-#pragma unroll
-      for (int k = 0; k < NG; k++) s_g[tid * NG + k] = 0.f;
     } else {
       s_bits[tid] = 0;
     }
@@ -600,16 +594,36 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
             mma_tf32(y0, y1, d2, d3, a0, a1, a2, a3, __float_as_uint(bc.z), __float_as_uint(bc.w));
           }
           // lane (g, t): d0/d1 = moments 2t, 2t+1 of hit g (t < 3) ; d2/d3 = colour sums 2t, 2t+1 of hit g (three channels:
-          // t = 0: 0, 1; t = 1: 2.  SIX: t < 3)
-          const uint32_t acc = s_g_addr + (4u * NG) * (uint32_t)__shfl_sync(FULL, my_e, g);
-          if (g < pend) {
-            if (t < 3) { red_shared_add_f32(acc + 8u * t, d0); red_shared_add_f32(acc + 8u * t + 4u, d1); }
-            if (SIX) {
-              if (t < 3) { red_shared_add_f32(acc + 24u + 8u * t, d2); red_shared_add_f32(acc + 28u + 8u * t, d3); }
-            } else {
-              if (t < 2) red_shared_add_f32(acc + 24u + 8u * t, d2);
-              if (t == 0) red_shared_add_f32(acc + 28u, d3);
-            }
+          // t = 0: 0, 1; t = 1: 2.  SIX: t < 3).  Gather hit g's outputs into lane (g, 0).
+          const float M00 = d0, M10 = d1;
+          const float M01 = __shfl_down_sync(FULL, d0, 1), M20 = __shfl_down_sync(FULL, d1, 1);
+          const float M11 = __shfl_down_sync(FULL, d0, 2), M02 = __shfl_down_sync(FULL, d1, 2);
+          const float c2 = __shfl_down_sync(FULL, d2, 1);
+          float c3 = 0.f, c4 = 0.f, c5 = 0.f;
+          if (SIX) { c3 = __shfl_down_sync(FULL, d3, 1); c4 = __shfl_down_sync(FULL, d2, 2); c5 = __shfl_down_sync(FULL, d3, 2); }
+          const int e = __shfl_sync(FULL, my_e, g);
+          if (t == 0 && g < pend) {
+            const float4 r0 = s_rec[F4 * e];
+            const float4 r1 = s_rec[F4 * e + 1];
+            const int id = __float_as_int(s_rec[F4 * e + 2].w);
+            const float X = r0.x - (tx0 + 7.5f), Y = r0.y - (ty0 + 7.5f);      // about the tile centre
+            const float Sx = fmaf(X, M00, -M10), Sy = fmaf(Y, M00, -M01);                       // sum wG dx, sum wG dy
+            const float Sxx = fmaf(X, fmaf(X, M00, -2.f * M10), M20);                           // sum wG dx^2
+            const float Syy = fmaf(Y, fmaf(Y, M00, -2.f * M01), M02);
+            const float Sxy = fmaf(X, fmaf(Y, M00, -M01), fmaf(-Y, M10, M11));                  // sum wG dx dy
+            float4 a, b;
+            a.x = -(r0.z * Sx + r0.w * Sy);          // d/dpx  (x log2e: the conic in the record is pre-scaled)
+            a.y = -(r1.x * Sy + r0.w * Sx);          // d/dpy  (x log2e)
+            a.z = -0.5f * Sxx;                       // d/dconic_x
+            a.w = -Sxy;                              // d/dconic_y
+            b.x = -0.5f * Syy;                       // d/dconic_z
+            b.y = M00 / r1.y;                        // d/dopacity = sum G dL/dalpha = sum wG / o
+            b.z = d2; b.w = d3;                      // d/drgb
+            float4* dst = reinterpret_cast<float4*>(dsplat + (int64_t)id * LGR_GRAD_FLOATS);
+            atomicAdd(dst, a);
+            atomicAdd(dst + 1, b);
+            if (SIX) atomicAdd(dst + 2, make_float4(c2, c3, c4, c5));      // d/db, d/dc3..5
+            else atomicAdd(reinterpret_cast<float*>(dst + 2), c2);
           }
           __syncwarp();
           pend = 0;
@@ -618,36 +632,6 @@ blend_bwd_kernel(View v, const int32_t* __restrict__ tile_start, const int32_t* 
       }
     }
     const int all_done = __syncthreads_and(done);      // B: every warp has left the walk
-    if (tid < cnt) {
-      const float* m = s_g + tid * NG;
-      const float M00 = m[0], M10 = m[1], M01 = m[2], M20 = m[3], M11 = m[4], M02 = m[5];
-      bool nz = (M00 != 0.f) | (M10 != 0.f) | (M01 != 0.f) | (M20 != 0.f) | (M11 != 0.f) | (M02 != 0.f) |
-                (m[6] != 0.f) | (m[7] != 0.f) | (m[8] != 0.f);
-      if (SIX) nz |= (m[NG - 3] != 0.f) | (m[NG - 2] != 0.f) | (m[NG - 1] != 0.f);
-      if (nz) {
-        const float4 r0 = s_rec[F4 * tid];
-        const float2 r1 = *reinterpret_cast<const float2*>(&s_rec[F4 * tid + 1]);
-        const int id = __float_as_int(s_rec[F4 * tid + 2].w);
-        const float X = r0.x - tcx, Y = r0.y - tcy;
-        const float Sx = fmaf(X, M00, -M10), Sy = fmaf(Y, M00, -M01);                       // sum wG dx, sum wG dy
-        const float Sxx = fmaf(X, fmaf(X, M00, -2.f * M10), M20);                           // sum wG dx^2
-        const float Syy = fmaf(Y, fmaf(Y, M00, -2.f * M01), M02);
-        const float Sxy = fmaf(X, fmaf(Y, M00, -M01), fmaf(-Y, M10, M11));                  // sum wG dx dy
-        float4 a, b;
-        a.x = -(r0.z * Sx + r0.w * Sy);          // d/dpx  (x log2e: the conic in the record is pre-scaled)
-        a.y = -(r1.x * Sy + r0.w * Sx);          // d/dpy  (x log2e)
-        a.z = -0.5f * Sxx;                       // d/dconic_x
-        a.w = -Sxy;                              // d/dconic_y
-        b.x = -0.5f * Syy;                       // d/dconic_z
-        b.y = M00 / r1.y;                        // d/dopacity = sum G dL/dalpha = sum wG / o
-        b.z = m[6]; b.w = m[7];                  // d/drgb
-        float4* dst = reinterpret_cast<float4*>(dsplat + (int64_t)id * LGR_GRAD_FLOATS);
-        atomicAdd(dst, a);
-        atomicAdd(dst + 1, b);
-        if (SIX) atomicAdd(dst + 2, make_float4(m[8], m[NG - 3], m[NG - 2], m[NG - 1]));      // d/db, d/dc3..5
-        else atomicAdd(reinterpret_cast<float*>(dst + 2), m[8]);
-      }
-    }
     base += BATCH;
     if (all_done || base >= n) break;
     cnt = min(BATCH, n - base);

@@ -5,7 +5,11 @@ compacted contribution list, lgr_view.contrib_count_d; n_contrib; tile_start):
   * the staged range of a full-list backward: whole 256-entry batches up to the one holding the tile's largest n_contrib;
   * the share of entries in that range that no sub-tile composited (every composited entry lies in that range, and the
     compacted list holds exactly those);
-  * batches per tile when the full list is staged, and when only the compacted list is (blend_bwd_kernel<true>).
+  * batches per tile when the full list is staged, and when only the compacted list is;
+  * what a backward that gives every 8x4 sub-tile its own warp would walk: the (warp, splat) hits, i.e.
+    the popcounts of the entries' sub-tile bytes summed, one vector RED triple per hit against one per compacted entry for a
+    per-tile reduction; per tile, the slowest warp's hits over the mean of its eight warps; the compacted entries each warp
+    reads (all of its tile's).
 
   python profiles/contrib_stats.py [--workload 10m]      (prints one JSON line)"""
 import argparse
@@ -55,6 +59,19 @@ def main():
     nz_staged = count[:len(lens)]
     assert (nz_staged <= staged).all()
     b_after = (nz_staged + BATCH - 1) // BATCH
+    # per (tile, sub-tile) hits of the compacted lists: bit w of an entry's low byte = sub-tile w composited it
+    entry = st.contrib_lists()[1].cpu().numpy().view(np.uint32)
+    ntiles = len(lens)
+    cnt = nz_staged
+    pos = np.repeat(start[:ntiles], cnt) + (np.arange(cnt.sum()) - np.repeat(np.cumsum(cnt) - cnt, cnt))
+    byte = (entry[pos] & 0xff).astype(np.uint8)
+    bits = np.unpackbits(byte[:, None], axis=1, bitorder='little')                  # (entries, 8): bit w
+    tile_of = np.repeat(np.arange(ntiles), cnt)
+    hits_tw = np.zeros((ntiles, 8), np.int64)
+    np.add.at(hits_tw, tile_of, bits.astype(np.int64))
+    busy = hits_tw.sum(axis=1) > 0
+    imb = hits_tw[busy].max(axis=1) / hits_tw[busy].mean(axis=1)
+    hits = int(hits_tw.sum())
     out = {
         'workload': args.workload, 'gpu': torch.cuda.get_device_name(), 'instances': int(lens.sum()),
         'tiles': int(len(lens)), 'tiles_with_entries': int(used.sum()),
@@ -63,6 +80,12 @@ def main():
         'staged_share_of_list': float(staged.sum() / max(lens.sum(), 1)),
         'batches_per_tile_before': {'mean': float(b_before[used].mean()), 'max': int(b_before.max()), 'total': int(b_before.sum())},
         'batches_per_tile_after': {'mean': float(b_after[used].mean()), 'max': int(b_after.max()), 'total': int(b_after.sum())},
+        'warp_hits': hits, 'warp_hits_per_entry': float(hits / max(int(cnt.sum()), 1)),
+        'vector_reds': {'per_warp_hit': 3 * hits, 'per_entry': 3 * int(cnt.sum())},
+        'slowest_warp_over_mean': {'mean': float(imb.mean()), 'p50': float(np.median(imb)), 'p90': float(np.percentile(imb, 90)),
+                                   'hit_weighted': float((hits_tw[busy].max(axis=1) * 8).sum() / max(hits, 1))},
+        'entries_per_warp_tile': {'mean': float(cnt[busy].mean()), 'max': int(cnt.max()),
+                                  'hits_per_warp_tile_mean': float(hits_tw[busy].mean())},
     }
     print(json.dumps(out))
 
