@@ -8,7 +8,8 @@
 // Exchange buffer of every rank (float offsets in lgr_shard_layout), R = ranks, cap = rows per (source, owner) pair:
 //   count  [R] int32        rows received from source s
 //   splat  [R*cap][12]      region s = rows pushed by source s, in ascending Gaussian index
-//   radii  [R*cap] int32    pixel radius of the row (0 = slot not in use this step)
+//   radii  [R*cap] int32    pixel radius of the row
+// Only the first count[s] rows of region s are in use this step; the other slots are never read or written.
 //   gid    [R*cap] int32    global Gaussian index of the row
 //   dsplat [R*cap][12]      RETURN: region o = 2D gradients sent back by band owner o, same row order as pushed
 //   weight [R*cap] uint32   RETURN: max alpha*T bits      pcount [R*cap] int32   RETURN: winner-pixel counts
@@ -169,7 +170,7 @@ shard_push_kernel(View v, ShardLayout L, int64_t n, int64_t gid_base, const floa
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// owner side: tile counts of the received rows, radii of unused slots cleared, gradient accumulators zeroed
+// owner side: tile counts of the received rows, their gradient and aux accumulators zeroed (unused slots untouched)
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SHARD_THREADS)
 shard_recv_count_kernel(View v, ShardLayout L, float* __restrict__ xbuf, float* __restrict__ dsplat,

@@ -165,9 +165,9 @@ def shard_layout(num_gaussians: int, world_size: int, rank: int):
     Footprint: every (source, owner) pair gets room for ALL of the source's Gaussians (cap = ceil(N/R) rows), because any
     view may send a whole shard into one band; a rank's buffer therefore holds R*cap ~ N rows of 112 bytes, plus the
     48-byte rows of `dsplat_rows`: ~1.6 GB per rank at 10 M Gaussians, ~8 GB at 50 M, independent of R.  Parameters,
-    gradients, optimiser state and all per-step scratch DO shrink with R; only this staging area does not.  The kernels
-    touch the count[s] used rows of a region, except the receive-side counting pass, which also walks the unused slots to
-    clear their stale radii."""
+    gradients, optimiser state and all per-step scratch DO shrink with R; only this staging area does not.  Every kernel
+    reads and writes only the count[s] used rows of a region: the unused slots keep whatever an earlier step left there
+    and are never read or written."""
     cap = owner_chunk(num_gaussians, world_size)
     rows = world_size * cap
     off = 0
