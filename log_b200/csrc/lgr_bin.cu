@@ -25,43 +25,24 @@ tile_scan_kernel(int ntiles, int32_t* __restrict__ tile_start /* out: starts[0..
                                                  for bin_partition, is never counted into: zero from the entry point's
                                                  memset) ; then ntiles ints: ids of long tiles */,
                  int32_t* __restrict__ meta, int small_cap) {
-  __shared__ int warp_sum[SCAN_THREADS / 32];
-  __shared__ int carry_s, maxl_s, nbig_s;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  if (tid == 0) { carry_s = 0; maxl_s = 0; nbig_s = 0; }
+  __shared__ int maxl_s, nbig_s;
+  if (threadIdx.x == 0) { maxl_s = 0; nbig_s = 0; }
   __syncthreads();
   int local_max = 0;
-  for (int base = 0; base < ntiles; base += SCAN_THREADS) {
-    const int i = base + tid;
-    const int c = (i < ntiles) ? cursor[i * CSTRIDE] + cursor[i * CSTRIDE + 1] : 0;
-    local_max = max(local_max, c);
-    int x = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) warp_sum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      int w = warp_sum[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-      warp_sum[lane] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    const int carry = carry_s;
-    const int excl = carry + (wid ? warp_sum[wid - 1] : 0) + x - c;
-    if (i < ntiles) {
-      tile_start[i] = excl; cursor[i * CSTRIDE] = 0;
-      if (c > small_cap) cursor[CSTRIDE * ntiles + atomicAdd(&nbig_s, 1)] = i;   // tiles the main sort launch cannot hold
-    }
-    __syncthreads();
-    if (tid == SCAN_THREADS - 1) carry_s = carry + warp_sum[31];
-    __syncthreads();
-  }
+  const int total = cta_exclusive_scan<SCAN_THREADS, 1>(
+      ntiles,
+      [&](int i, int) {
+        const int c = cursor[i * CSTRIDE] + cursor[i * CSTRIDE + 1];
+        local_max = max(local_max, c);
+        if (c > small_cap) cursor[CSTRIDE * ntiles + atomicAdd(&nbig_s, 1)] = i;   // tiles the main sort launch cannot hold
+        return c;
+      },
+      [&](int i, int, int excl) { tile_start[i] = excl; cursor[i * CSTRIDE] = 0; }).v[0];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) local_max = max(local_max, __shfl_xor_sync(0xffffffffu, local_max, o));
-  if (lane == 0) atomicMax(&maxl_s, local_max);
+  if ((threadIdx.x & 31) == 0) atomicMax(&maxl_s, local_max);
   __syncthreads();
-  if (tid == 0) { tile_start[ntiles] = carry_s; meta[0] = carry_s; meta[1] = maxl_s; meta[5] = nbig_s; }
+  if (threadIdx.x == 0) { tile_start[ntiles] = total; meta[0] = total; meta[1] = maxl_s; meta[5] = nbig_s; }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -97,26 +78,6 @@ __device__ __forceinline__ unsigned long long composite(uint32_t k, uint32_t v) 
 
 int part_smem_bytes(int rows) { return 3 * (int)sizeof(int32_t) * max(rows, 1); }
 
-// Exclusive scan of in[0,len) into out (in == out allowed).  Block-wide, convergent; `wsum` holds BIN_THREADS/32 ints.
-__device__ __forceinline__ void block_exclusive_scan(const int* in, int* out, int len, int* wsum) {
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  int carry = 0;
-  for (int base = 0; base < len; base += BIN_THREADS) {
-    const int c = base + tid < len ? in[base + tid] : 0;
-    int x = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[wid] = x;
-    __syncthreads();
-    int before = carry, all = carry;
-#pragma unroll
-    for (int w = 0; w < BIN_THREADS / 32; w++) { if (w < wid) before += wsum[w]; all += wsum[w]; }
-    if (base + tid < len) out[base + tid] = before + x - c;
-    carry = all;
-    __syncthreads();
-  }
-}
-
 __global__ void __launch_bounds__(BIN_THREADS, 6)
 bin_partition_kernel(View v, int64_t n, const float* __restrict__ splat, const int32_t* __restrict__ radii,
                      const int32_t* __restrict__ tile_start, int32_t* __restrict__ cursor, unsigned long long* __restrict__ stage,
@@ -132,7 +93,6 @@ bin_partition_kernel(View v, int64_t n, const float* __restrict__ splat, const i
   __shared__ int32_t s_tile[PART_CAP];
   __shared__ uint16_t s_perm[PART_CAP];
   __shared__ int s_fill;
-  __shared__ int s_wsum[BIN_THREADS / 32];
   __shared__ int64_t s_first[LGR_SHARD_MAX_RANKS + 1];
   const int rows = v.row1 - v.row0, lane = threadIdx.x & 31;
   int32_t* r_cnt = row_tab;
@@ -161,7 +121,7 @@ bin_partition_kernel(View v, int64_t n, const float* __restrict__ splat, const i
       const int c = r_cnt[r];
       if (c > 0) r_base[r] = tile_start[r * v.gx] + atomicAdd(cursor + r * v.gx * CSTRIDE + 2, c);
     }
-    block_exclusive_scan(r_cnt, r_off, rows, s_wsum);
+    cta_exclusive_scan<BIN_THREADS, 1>(rows, [&](int r, int) { return r_cnt[r]; }, [&](int r, int, int off) { r_off[r] = off; });
     for (int r = threadIdx.x; r < rows; r += BIN_THREADS) r_base[r] -= r_off[r];      // run base minus the group's offset
     __syncthreads();
     for (int e = threadIdx.x; e < held; e += BIN_THREADS) s_perm[atomicAdd(&r_off[s_tile[e] / v.gx], 1)] = (uint16_t)e;
@@ -222,9 +182,7 @@ bin_partition_kernel(View v, int64_t n, const float* __restrict__ splat, const i
       const int w = x1 - x0, cnt = live ? w * (y1 - y0) : 0;
       // Small splats (at most 4 tiles): held in shared memory, slots handed out per warp (one shared atomic per warp).
       const int mine = cnt <= 4 ? cnt : 0;
-      int incl = mine;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += y; }
+      const int incl = warp_inclusive_scan(mine);
       int wbase = 0;
       if (lane == 31 && incl > 0) wbase = atomicAdd(&s_fill, incl);
       wbase = __shfl_sync(0xffffffffu, wbase, 31);
@@ -664,49 +622,20 @@ pc_block_count_kernel(int64_t n, const int32_t* __restrict__ count, int32_t* __r
 
 __global__ void __launch_bounds__(1024)
 pc_scan_kernel(int nb, int32_t* __restrict__ blk /* [0,nb) counts -> [nb, 2nb] exclusive prefix */, int32_t* __restrict__ num_out) {
-  __shared__ int warp_sum[32];
-  __shared__ int carry_s;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  if (tid == 0) carry_s = 0;
-  __syncthreads();
-  for (int base = 0; base < nb; base += 1024) {
-    const int b = base + tid;
-    const int c = b < nb ? blk[b] : 0;
-    int x = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) warp_sum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      int w = warp_sum[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-      warp_sum[lane] = w;
-    }
-    __syncthreads();
-    const int carry = carry_s;
-    if (b < nb) blk[nb + b] = carry + (wid ? warp_sum[wid - 1] : 0) + x - c;
-    __syncthreads();
-    if (tid == 1023) carry_s = carry + warp_sum[31];
-    __syncthreads();
-  }
-  if (tid == 0) { blk[2 * nb] = carry_s; *num_out = carry_s; }
+  const int total = cta_exclusive_scan<1024, 1>(nb, [&](int b, int) { return blk[b]; },
+                                                [&](int b, int, int pre) { blk[nb + b] = pre; }).v[0];
+  if (threadIdx.x == 0) { blk[2 * nb] = total; *num_out = total; }
 }
 
 __global__ void __launch_bounds__(PC_THREADS)
 pc_compact_kernel(int64_t n, const int32_t* __restrict__ count, const int32_t* __restrict__ blk, int nb,
                   int32_t* __restrict__ ids_out, int32_t* __restrict__ counts_out) {
-  __shared__ int wsum[PC_THREADS / 32];
+  __shared__ int wcnt[PC_THREADS / 32];
   const int64_t i = (int64_t)blockIdx.x * PC_THREADS + threadIdx.x;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int c = i < n ? count[i] : 0;
-  const unsigned bal = __ballot_sync(0xffffffffu, c > 0);
-  if (lane == 0) wsum[wid] = __popc(bal);
-  __syncthreads();
-  int base = blk[nb + blockIdx.x];
-  for (int w = 0; w < wid; w++) base += wsum[w];
+  const int rank = cta_ballot_rank<PC_THREADS>(c > 0, wcnt).rank;
   if (c > 0) {
-    const int pos = base + __popc(bal & ((1u << lane) - 1u));
+    const int pos = blk[nb + blockIdx.x] + rank;
     ids_out[pos] = (int32_t)i;
     counts_out[pos] = c;
   }

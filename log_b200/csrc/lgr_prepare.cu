@@ -10,8 +10,8 @@
 //   split    one thread per walk entry: LoG's leaf / node rule (:244-251), two order-preserving lists
 //
 // Every compaction is the pattern of lgr_tree.cu: a fixed grid of grid-stride loops over a count that may live on the
-// device, per-chunk counts, a one-CTA exclusive scan, then chunk prefix + ballot rank.  The counts land in the (int64)
-// result vector the host reads once.
+// device, per-chunk counts, a one-CTA exclusive scan (cta_exclusive_scan), then chunk prefix + ballot rank
+// (cta_ballot_rank).  The counts land in the (int64) result vector the host reads once.
 #include "lgr_common.cuh"
 
 namespace lgr {
@@ -21,7 +21,6 @@ constexpr int PREP_THREADS = COMPACT_CHUNK;
 #define LGR_TREE_GRID 528               // 4 CTAs per SM on the 132 SMs of an H100 SXM; grid-stride loops cover any size
 #endif
 constexpr int PREP_GRID = LGR_TREE_GRID;
-constexpr unsigned PREP_FULL = 0xffffffffu;
 
 enum PrepMode { CULL_ROOTS = 0, CULL_POINTS = 1, MERGE = 2, SPLIT = 3 };
 
@@ -99,44 +98,13 @@ prep_classify_kernel(PrepArgs a, int64_t n_host, const int64_t* __restrict__ n_d
 __global__ void __launch_bounds__(1024)
 prep_scan_kernel(int64_t n_host, const int64_t* __restrict__ n_d, int32_t* __restrict__ chunk_cnt, int64_t* __restrict__ total_a,
                  int64_t* __restrict__ total_b) {
-  __shared__ __align__(16) int wsum[2][32];
-  __shared__ int carry[2];
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int64_t n = n_d ? *n_d : n_host;
-  const int nchunks = (int)((n + PREP_THREADS - 1) / PREP_THREADS);
-  if (tid < 2) carry[tid] = 0;
-  __syncthreads();
-  for (int base = 0; base < nchunks; base += 1024) {
-    const int b = base + tid;
-    int c[2], x[2];
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      c[k] = b < nchunks ? chunk_cnt[2 * b + k] : 0;
-      x[k] = c[k];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(PREP_FULL, x[k], o); if (lane >= o) x[k] += y; }
-      if (lane == 31) wsum[k][wid] = x[k];
-    }
-    __syncthreads();
-    if (wid < 2) {
-      int w = wsum[wid][lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(PREP_FULL, w, o); if (lane >= o) w += y; }
-      wsum[wid][lane] = w;
-    }
-    __syncthreads();
-    const int c0 = carry[0], c1 = carry[1];
-    if (b < nchunks) {
-      chunk_cnt[2 * b] = c0 + (wid ? wsum[0][wid - 1] : 0) + x[0] - c[0];
-      chunk_cnt[2 * b + 1] = c1 + (wid ? wsum[1][wid - 1] : 0) + x[1] - c[1];
-    }
-    __syncthreads();
-    if (tid == 0) { carry[0] = c0 + wsum[0][31]; carry[1] = c1 + wsum[1][31]; }
-    __syncthreads();
-  }
-  if (tid == 0) {
-    if (total_a) *total_a = carry[0];
-    if (total_b) *total_b = carry[1];
+  const ScanTotals<2> t = cta_exclusive_scan<1024, 2>((int)((n + PREP_THREADS - 1) / PREP_THREADS),
+                                                      [&](int b, int k) { return chunk_cnt[2 * b + k]; },
+                                                      [&](int b, int k, int pre) { chunk_cnt[2 * b + k] = pre; });
+  if (threadIdx.x == 0) {
+    if (total_a) *total_a = t.v[0];
+    if (total_b) *total_b = t.v[1];
   }
 }
 
@@ -150,21 +118,14 @@ prep_scatter_kernel(int64_t n_host, const int64_t* __restrict__ n_d, const Cand*
                     int64_t* __restrict__ out_b, const int64_t* __restrict__ total_a, int pad_a) {
   __shared__ __align__(16) int wa[PREP_THREADS / 32];
   __shared__ __align__(16) int wb[PREP_THREADS / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t n = n_d ? *n_d : n_host;
   const int64_t nchunks = (n + PREP_THREADS - 1) / PREP_THREADS;
   for (int64_t chunk = blockIdx.x; chunk < nchunks; chunk += gridDim.x) {
     const int64_t slot = chunk * PREP_THREADS + threadIdx.x;
     const int f = slot < n ? bits[slot] : 0;
-    const unsigned ba = __ballot_sync(PREP_FULL, f & 1), bb = __ballot_sync(PREP_FULL, f & 2);
-    if (lane == 0) { wa[wid] = __popc(ba); wb[wid] = __popc(bb); }
-    __syncthreads();
-    int pa = chunk_pre[2 * chunk], pb = chunk_pre[2 * chunk + 1];
-    for (int w = 0; w < wid; w++) { pa += wa[w]; pb += wb[w]; }
-    const unsigned lt = (1u << lane) - 1u;
-    if (f & 1) out_a[pa + __popc(ba & lt)] = cand ? (int64_t)cand[slot] : slot;
-    if (f & 2) out_b[pb + __popc(bb & lt)] = cand ? (int64_t)cand[slot] : slot;
-    __syncthreads();
+    const int ra = cta_ballot_rank<PREP_THREADS>(f & 1, wa).rank, rb = cta_ballot_rank<PREP_THREADS>(f & 2, wb).rank;
+    if (f & 1) out_a[chunk_pre[2 * chunk] + ra] = cand ? (int64_t)cand[slot] : slot;
+    if (f & 2) out_b[chunk_pre[2 * chunk + 1] + rb] = cand ? (int64_t)cand[slot] : slot;
   }
   if (pad_a) {
     const int64_t t = *total_a;

@@ -98,8 +98,7 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
   constexpr bool USE_SH = C == Colour::SH, LOG_SH = C == Colour::LOG_SH, SIX = C == Colour::RGB6;
   __shared__ float sV[16], sP[16], sCam[3];
   __shared__ float sWf;
-  __shared__ unsigned sStock[PROJ_THREADS / 32];
-  __shared__ int sVis[PROJ_THREADS / 32];
+  __shared__ int sWcnt[PROJ_THREADS / 32];      // band mode: the per-warp table of the two compactions
   if (threadIdx.x < 16) { sV[threadIdx.x] = v.view[threadIdx.x]; sP[threadIdx.x] = v.proj[threadIdx.x]; }
   if (threadIdx.x == 32) {
     float a = 0.f;
@@ -151,18 +150,11 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     // The survivors are a minority scattered over all warps: compact them inside the CTA so that the heavy projection
     // below runs on dense warps (it is instruction bound, ~400 instructions per Gaussian).
     __shared__ int sSurv[PROJ_THREADS];
-    __shared__ int sWcnt[PROJ_THREADS / 32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     if (!work && i < n) radii[i] = 0;
-    const unsigned bal = __ballot_sync(0xffffffffu, work);
-    if (lane == 0) sWcnt[wid] = __popc(bal);
-    __syncthreads();
-    int base = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < PROJ_THREADS / 32; w++) { const int c = sWcnt[w]; if (w < wid) base += c; total += c; }
-    if (work) sSurv[base + __popc(bal & ((1u << lane) - 1u))] = threadIdx.x;
-    __syncthreads();
-    work = threadIdx.x < total;
+    const CtaRank r = cta_ballot_rank<PROJ_THREADS>(work, sWcnt);
+    if (work) sSurv[r.rank] = threadIdx.x;
+    __syncthreads();      // also orders the reads of sWcnt before the band ids' ranking below
+    work = threadIdx.x < r.total;
     i = work ? (int64_t)blockIdx.x * PROJ_THREADS + sSurv[threadIdx.x] : n;
   }
   bool big_splat = false;      // covers more than 4 tiles: counted by the whole warp after the divergent part
@@ -274,32 +266,12 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
   }
   warp_count_big_tiles(v, tile_count, big_splat, bx0, by0, bx1, by1);
   if (v.num_owners > 0) {      // atomics-free compaction of the ids that reach the band into this CTA's segment
-    __shared__ int sCnt[PROJ_THREADS / 32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const unsigned bal = __ballot_sync(0xffffffffu, in_band);
-    if (lane == 0) sCnt[wid] = __popc(bal);
-    __syncthreads();
-    int base = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < PROJ_THREADS / 32; w++) { const int c = sCnt[w]; if (w < wid) base += c; total += c; }
-    if (in_band) v.band_ids[(int64_t)blockIdx.x * PROJ_THREADS + base + __popc(bal & ((1u << lane) - 1u))] = (int)i;
-    if (threadIdx.x == 0) v.band_blk[blockIdx.x] = total;
-    __syncthreads();
+    const CtaRank r = cta_ballot_rank<PROJ_THREADS>(in_band, sWcnt);
+    if (in_band) v.band_ids[(int64_t)blockIdx.x * PROJ_THREADS + r.rank] = (int)i;
+    if (threadIdx.x == 0) v.band_blk[blockIdx.x] = r.total;
   }
   // block statistics: D by the stock rule, number of visible Gaussians (one atomic pair per CTA)
-  {
-    const unsigned st_w = __reduce_add_sync(0xffffffffu, (unsigned)stock_tiles);      // < 2^32 per warp
-    const int vis_w = __popc(__ballot_sync(0xffffffffu, rad_out > 0));
-    if ((threadIdx.x & 31) == 0) { sStock[threadIdx.x >> 5] = st_w; sVis[threadIdx.x >> 5] = vis_w; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned long long a = 0; int b = 0;
-#pragma unroll
-      for (int w = 0; w < PROJ_THREADS / 32; w++) { a += sStock[w]; b += sVis[w]; }
-      if (a) atomicAdd(reinterpret_cast<unsigned long long*>(meta + 2), a);
-      if (b) atomicAdd(meta + 4, b);
-    }
-  }
+  cta_add_view_stats<PROJ_THREADS>((unsigned)stock_tiles, rad_out > 0 ? 1 : 0, meta);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -594,37 +566,14 @@ project_bwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024)
 band_scan_kernel(View v) {
-  __shared__ int warp_sum[32];
-  __shared__ int carry_s;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, B = v.band_blocks;
-  if (tid == 0) carry_s = 0;
-  __syncthreads();
-  for (int base = 0; base < B; base += 1024) {
-    const int b = base + tid;
-    const int c = b < B ? v.band_blk[b] : 0;
-    int x = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) warp_sum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      int w = warp_sum[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-      warp_sum[lane] = w;
-    }
-    __syncthreads();
-    const int carry = carry_s;
-    if (b < B) v.band_blk[B + b] = carry + (wid ? warp_sum[wid - 1] : 0) + x - c;
-    __syncthreads();
-    if (tid == 1023) carry_s = carry + warp_sum[31];
-    __syncthreads();
-  }
-  if (tid == 0) v.band_blk[2 * B] = carry_s;
+  const int B = v.band_blocks;
+  const int total = cta_exclusive_scan<1024, 1>(B, [&](int b, int) { return v.band_blk[b]; },
+                                                [&](int b, int, int pre) { v.band_blk[B + b] = pre; }).v[0];
+  if (threadIdx.x == 0) v.band_blk[2 * B] = total;
   __syncthreads();
   // owner o covers CTAs [o*cpb, (o+1)*cpb): total = prefix difference
   const int cpb = v.owner_chunk / PROJ_THREADS;
-  for (int o = tid; o < v.num_owners; o += 1024) {
+  for (int o = threadIdx.x; o < v.num_owners; o += 1024) {
     const int b0 = min(B, o * cpb), b1 = min(B, (o + 1) * cpb);
     v.band_count[o] = v.band_blk[B + b1] - v.band_blk[B + b0];
   }

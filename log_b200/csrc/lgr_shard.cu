@@ -89,36 +89,11 @@ shard_count_kernel(View v, int R, int64_t n, const float* __restrict__ splat, co
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024)
 shard_scan_kernel(ShardLayout L, int B, int32_t* __restrict__ send_blk, void* const* __restrict__ peer_base) {
-  __shared__ int warp_sum[32];
-  __shared__ int carry_s;
-  const int o = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int o = blockIdx.x;
   const int32_t* cnt = send_blk + (int64_t)o * B;
   int32_t* pre = send_blk + (int64_t)(L.R + o) * B;
-  if (tid == 0) carry_s = 0;
-  __syncthreads();
-  for (int base = 0; base < B; base += 1024) {
-    const int b = base + tid;
-    const int c = b < B ? cnt[b] : 0;
-    int x = c;
-#pragma unroll
-    for (int k = 1; k < 32; k <<= 1) { const int y = __shfl_up_sync(FULLMASK, x, k); if (lane >= k) x += y; }
-    if (lane == 31) warp_sum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      int w = warp_sum[lane];
-#pragma unroll
-      for (int k = 1; k < 32; k <<= 1) { const int y = __shfl_up_sync(FULLMASK, w, k); if (lane >= k) w += y; }
-      warp_sum[lane] = w;
-    }
-    __syncthreads();
-    const int carry = carry_s;
-    if (b < B) pre[b] = carry + (wid ? warp_sum[wid - 1] : 0) + x - c;
-    __syncthreads();
-    if (tid == 1023) carry_s = carry + warp_sum[31];
-    __syncthreads();
-  }
-  if (tid == 0) {
-    const int total = carry_s;
+  const int total = cta_exclusive_scan<1024, 1>(B, [&](int b, int) { return cnt[b]; }, [&](int b, int, int p) { pre[b] = p; }).v[0];
+  if (threadIdx.x == 0) {
     send_blk[(int64_t)2 * L.R * B + o] = total;
     reinterpret_cast<int32_t*>(reinterpret_cast<float*>(peer_base[o]) + L.off_count)[L.me] = total;
   }
@@ -176,8 +151,6 @@ __global__ void __launch_bounds__(SHARD_THREADS)
 shard_recv_count_kernel(View v, ShardLayout L, float* __restrict__ xbuf, float* __restrict__ dsplat,
                         int32_t* __restrict__ tile_count, int32_t* __restrict__ meta, float* __restrict__ pw_rows,
                         int32_t* __restrict__ pc_rows) {
-  __shared__ __align__(16) unsigned sStock[SHARD_WARPS];
-  __shared__ __align__(16) int sVis[SHARD_WARPS];
   // strides over the USED rows (the first count[s] rows of region s); unused rows are never touched -- every later kernel
   // of the band render follows the same map (View::region_count)
   __shared__ int64_t s_first[LGR_SHARD_MAX_RANKS + 1];
@@ -208,17 +181,7 @@ shard_recv_count_kernel(View v, ShardLayout L, float* __restrict__ xbuf, float* 
     }
     warp_count_big_tiles(v, tile_count, big_splat, bx0, by0, bx1, by1);
   }
-  const unsigned st_w = __reduce_add_sync(FULLMASK, stock);
-  const int vis_w = __reduce_add_sync(FULLMASK, vis);
-  if ((threadIdx.x & 31) == 0) { sStock[threadIdx.x >> 5] = st_w; sVis[threadIdx.x >> 5] = vis_w; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long a = 0; int b = 0;
-#pragma unroll
-    for (int w = 0; w < SHARD_WARPS; w++) { a += sStock[w]; b += sVis[w]; }
-    if (a) atomicAdd(reinterpret_cast<unsigned long long*>(meta + 2), a);
-    if (b) atomicAdd(meta + 4, b);
-  }
+  cta_add_view_stats<SHARD_THREADS>(stock, vis, meta);
 }
 
 // ---------------------------------------------------------------------------------------------------------

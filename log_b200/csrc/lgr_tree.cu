@@ -26,7 +26,6 @@ constexpr int TREE_THREADS = 256;
 #define LGR_TREE_GRID 528               // 4 CTAs per SM on the 132 SMs of an H100 SXM; grid-stride loops cover any size
 #endif
 constexpr int TREE_GRID = LGR_TREE_GRID;
-constexpr unsigned TREE_FULL = 0xffffffffu;
 
 
 // state[0] frontier size   state[1] output size   state[2] kept (this level)   state[3] descending (this level)
@@ -81,42 +80,11 @@ tree_classify_kernel(TreeArgs a, const int64_t* __restrict__ roots, const int32_
 // exclusive scan of the (kept, descending) chunk counts in place; totals into state[2], state[3]
 __global__ void __launch_bounds__(1024)
 tree_scan_kernel(int C_or_one, int32_t* __restrict__ state, int32_t* __restrict__ chunk_cnt) {
-  __shared__ __align__(16) int wsum[2][32];
-  __shared__ int carry[2];
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int64_t nslots = (int64_t)state[ST_FRONT] * C_or_one;
-  const int nchunks = (int)((nslots + TREE_THREADS - 1) / TREE_THREADS);
-  if (tid < 2) carry[tid] = 0;
-  __syncthreads();
-  for (int base = 0; base < nchunks; base += 1024) {
-    const int b = base + tid;
-    int c[2], x[2];
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      c[k] = b < nchunks ? chunk_cnt[2 * b + k] : 0;
-      x[k] = c[k];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(TREE_FULL, x[k], o); if (lane >= o) x[k] += y; }
-      if (lane == 31) wsum[k][wid] = x[k];
-    }
-    __syncthreads();
-    if (wid < 2) {
-      int w = wsum[wid][lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(TREE_FULL, w, o); if (lane >= o) w += y; }
-      wsum[wid][lane] = w;
-    }
-    __syncthreads();
-    const int c0 = carry[0], c1 = carry[1];
-    if (b < nchunks) {
-      chunk_cnt[2 * b] = c0 + (wid ? wsum[0][wid - 1] : 0) + x[0] - c[0];
-      chunk_cnt[2 * b + 1] = c1 + (wid ? wsum[1][wid - 1] : 0) + x[1] - c[1];
-    }
-    __syncthreads();
-    if (tid == 0) { carry[0] = c0 + wsum[0][31]; carry[1] = c1 + wsum[1][31]; }
-    __syncthreads();
-  }
-  if (tid == 0) { state[2] = carry[0]; state[3] = carry[1]; }
+  const ScanTotals<2> t = cta_exclusive_scan<1024, 2>((int)((nslots + TREE_THREADS - 1) / TREE_THREADS),
+                                                      [&](int b, int k) { return chunk_cnt[2 * b + k]; },
+                                                      [&](int b, int k, int pre) { chunk_cnt[2 * b + k] = pre; });
+  if (threadIdx.x == 0) { state[2] = t.v[0]; state[3] = t.v[1]; }
 }
 
 // stable compaction: kept candidates append to `out`, descending ones form the next frontier
@@ -126,22 +94,15 @@ tree_scatter_kernel(int C_or_one, const int32_t* __restrict__ state, const int32
                     int32_t* __restrict__ next_front) {
   __shared__ __align__(16) int wk[TREE_THREADS / 32];
   __shared__ __align__(16) int wn[TREE_THREADS / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t nslots = (int64_t)state[ST_FRONT] * C_or_one;
   const int64_t nchunks = (nslots + TREE_THREADS - 1) / TREE_THREADS;
   const int64_t out_base = state[ST_OUT];
   for (int64_t chunk = blockIdx.x; chunk < nchunks; chunk += gridDim.x) {
     const int64_t slot = chunk * TREE_THREADS + threadIdx.x;
     const int f = slot < nslots ? flags[slot] : 0;
-    const unsigned bk = __ballot_sync(TREE_FULL, f & 1), bn = __ballot_sync(TREE_FULL, f & 2);
-    if (lane == 0) { wk[wid] = __popc(bk); wn[wid] = __popc(bn); }
-    __syncthreads();
-    int pk = chunk_pre[2 * chunk], pn = chunk_pre[2 * chunk + 1];
-    for (int w = 0; w < wid; w++) { pk += wk[w]; pn += wn[w]; }
-    const unsigned lt = (1u << lane) - 1u;
-    if (f & 1) out[out_base + pk + __popc(bk & lt)] = cand[slot];
-    if (f & 2) next_front[pn + __popc(bn & lt)] = cand[slot];
-    __syncthreads();
+    const int rk = cta_ballot_rank<TREE_THREADS>(f & 1, wk).rank, rn = cta_ballot_rank<TREE_THREADS>(f & 2, wn).rank;
+    if (f & 1) out[out_base + chunk_pre[2 * chunk] + rk] = cand[slot];
+    if (f & 2) next_front[chunk_pre[2 * chunk + 1] + rn] = cand[slot];
   }
 }
 

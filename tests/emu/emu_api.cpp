@@ -7,6 +7,7 @@ int launch_tile_scan(int, int32_t*, int32_t*, int32_t*, bool, cudaStream_t);
 int launch_bin_and_sort(const View&, int64_t, int64_t, int, int, const float*, const int32_t*, int32_t*, int32_t*,
                         uint32_t*, uint32_t*, uint32_t*, int32_t*, int32_t*, cudaStream_t);
 int launch_point_compact(int64_t, const int32_t*, int32_t*, int32_t*, int32_t*, int32_t*, cudaStream_t);
+int launch_band_scan(const View&, cudaStream_t);
 int sort_smem_capacity();
 int launch_shard_send(const View&, const ShardLayout&, int64_t, int64_t, const float*, const int32_t*, int32_t*, void* const*,
                       cudaStream_t);
@@ -43,6 +44,9 @@ int emu_bin_and_sort(const lgr_view* view, int64_t n, int64_t num_instances, int
   return launch_bin_and_sort(make_view(view, n), n, num_instances, max_tile_len, num_long_tiles, splat, radii, const_cast<int32_t*>(tile_start),
                              tile_cursor, inst_key, inst_val, inst_tmp, sorted_ids, nullptr, nullptr);
 }
+
+// band mode: band_blk_d[0, B) holds the per-CTA list lengths of n Gaussians (B = ceil(n / 256)), as project_fwd leaves them
+int emu_band_scan(const lgr_view* view, int64_t n) { return launch_band_scan(make_view(view, n), nullptr); }
 
 int emu_point_compact(int64_t n, const int32_t* count, int32_t* scratch, int32_t* ids, int32_t* counts, int32_t* num) {
   return launch_point_compact(n, count, scratch, ids, counts, num, nullptr);

@@ -8,6 +8,11 @@ equality (the shard-mode gradients, which add in another order, excepted), and e
 crosses the boundary it exists for.
 
   boundary (constant in log_b200/csrc)                              test
+  tile_scan_kernel carry: > 1024 tiles                              test_tile_scan_past_one_scan_pass_emulated, test_tile_lists.py::test_ten_million_1080p
+  band_scan_kernel carry: > 1024 x 256 Gaussians in band mode       test_band_scan_past_one_scan_pass_emulated
+  prep_scan_kernel carry, prepare cull: > 1024 x 256 points         test_compactions_past_one_scan_pass*[prepare_cull]
+  prep_scan_kernel carry, densify plan: > 1024 x 256 rows           test_compactions_past_one_scan_pass*[densify_plan]
+  prep_scan_kernel carry, step order: > 1024 x 256 Gaussians        test_compactions_past_one_scan_pass*[step_order]
   shard_scan_kernel carry: a source owns > 1024 x 256 rows          test_shard_exchange_scan_carry_emulated, test_shard_mode_at_metric_size
   region-strided kernels: an owner receives > 2112 x 256 rows       test_shard_mode_at_metric_size (emulator: grid of 2)
   equal-depth ties inside one tile in shard mode                    test_shard_mode_at_metric_size
@@ -35,7 +40,9 @@ from test_emulated_kernels import emu                                  # noqa: E
 from test_tree_traverse import stand_ins                               # noqa: E402
 from util import device, f32_camera, run_gpu, settings_from_camera     # noqa: E402
 
-SCAN_PASS = 1024            # entries per pass of a one-CTA scan (shard_scan, tree_scan, pc_scan)
+SCAN_PASS = 1024            # entries per pass of a one-CTA scan (tile_scan, band_scan, prep_scan, shard_scan, tree_scan, pc_scan)
+COMPACT_CHUNK = 256         # lgr_common.cuh: slots per chunk of the compactions behind prep_scan
+BAND_PER_CTA = 256          # lgr_project.cu PROJ_THREADS: one band-list length per CTA
 SHARD_ROWS_PER_CTA = 256    # lgr_shard.cu SHARD_THREADS
 TREE_SLOTS_PER_CTA = 256    # lgr_tree.cu TREE_THREADS
 PC_PER_BLOCK = 1024         # lgr_bin.cu PC_THREADS
@@ -82,6 +89,149 @@ def test_point_compaction_past_one_scan_pass_emulated(emulated_backend, n):
 @pytest.mark.parametrize('n', [1 << 20, (1 << 20) + 1, 1024 * 1025 + 3, 10_000_000])
 def test_point_compaction_past_one_scan_pass(built, n):
     check_point_compaction(n)
+
+
+# ---- tile scan -------------------------------------------------------------------------------------------------------
+def test_tile_scan_past_one_scan_pass_emulated(emu):
+    """2 600 tiles: three passes of the scan.  Each tile's count is split over its two counters, and about 1 % of the
+    tiles are longer than the main sort launch holds (the long-tile list behind the cursors)."""
+    gx, gy = 65, 40
+    n = gx * gy
+    assert n > 2 * SCAN_PASS, 'case no longer reaches the intended route'
+    rng = np.random.default_rng(21)
+    a, b = rng.integers(0, 60, n), rng.integers(0, 60, n)
+    a[rng.random(n) < 0.01] += SORT_CAP_SMALL
+    c = a + b
+    cursor = np.full(TEK.CSTRIDE * n + n, -7, np.int32)
+    cursor[0:TEK.CSTRIDE * n:TEK.CSTRIDE], cursor[1:TEK.CSTRIDE * n:TEK.CSTRIDE] = a, b
+    tile_start, meta = np.full(n + 1, -1, np.int32), np.zeros(8, np.int32)
+    assert emu.emu_tile_scan(ctypes.byref(TEK.make_view(16 * gy, 16 * gx)), TEK.P(tile_start), TEK.P(cursor), TEK.P(meta)) == 0
+    assert np.array_equal(tile_start, np.concatenate([[0], np.cumsum(c)]))
+    assert (meta[0], meta[1], meta[5]) == (c.sum(), c.max(), (c > SORT_CAP_SMALL).sum())
+    assert np.array_equal(np.sort(cursor[TEK.CSTRIDE * n:TEK.CSTRIDE * n + meta[5]]), np.nonzero(c > SORT_CAP_SMALL)[0])
+    assert (cursor[0:TEK.CSTRIDE * n:TEK.CSTRIDE] == 0).all()
+
+
+
+# ---- band scan --------------------------------------------------------------------------------------------------------
+def test_band_scan_past_one_scan_pass_emulated(emu):
+    """Band mode's per-CTA list lengths of 300 000 Gaussians over 3 owners (1 172 CTAs): the row offsets and per-owner
+    totals after a second pass of the scan."""
+    from log_b200 import sharded
+    n, owners = 300_000, 3
+    B = -(-n // BAND_PER_CTA)
+    assert B > SCAN_PASS, 'case no longer reaches the intended route'
+    rng = np.random.default_rng(22)
+    blk = np.full(2 * B + 1, -1, np.int32)
+    blk[:B] = rng.integers(0, BAND_PER_CTA + 1, B) * (rng.random(B) < 0.7)
+    count = np.full(owners, -1, np.int32)
+    v = TEK.make_view(64, 64)
+    v.num_owners, v.band_blk_d, v.band_count_d = owners, blk.ctypes.data, count.ctypes.data
+    emu.emu_band_scan.restype = ctypes.c_int
+    emu.emu_band_scan.argtypes = [ctypes.c_void_p, ctypes.c_int64]
+    assert emu.emu_band_scan(ctypes.byref(v), n) == 0
+    pre = np.concatenate([[0], np.cumsum(blk[:B])])
+    assert np.array_equal(blk[B:], pre)
+    parts = sharded.owner_partition(n, owners)
+    assert all(lo % BAND_PER_CTA == 0 for lo, _ in parts)
+    assert np.array_equal(count, [blk[lo // BAND_PER_CTA:-(-hi // BAND_PER_CTA)].sum() for lo, hi in parts])
+
+
+# ---- order-preserving compactions (lgr_prepare.cu): chunk counts, prep_scan, ballot-rank scatter -----------------------
+COMPACT_SLOTS = SCAN_PASS * COMPACT_CHUNK + 37_000       # chunk counts: a second pass of the scan
+
+
+def mixed_flags(n, seed):
+    """~60 % set, plus whole empty and whole full chunks on both sides of the first pass boundary of the chunk scan."""
+    rng = np.random.default_rng(seed)
+    f = rng.random(n) < 0.6
+    for k, fill in ((SCAN_PASS - 2, False), (SCAN_PASS - 1, True), (SCAN_PASS, False), (SCAN_PASS + 1, True)):
+        f[k * COMPACT_CHUNK:(k + 1) * COMPACT_CHUNK] = fill
+    return f
+
+
+def check_prepare_cull(lib, dev):
+    """The base stage's cull: the in-range ids are the flagged points in id order (the flags are the kernel's own)."""
+    from log_b200 import _capi
+    from log_b200.rasterizer import _ptr
+    n = COMPACT_SLOTS
+    rng = np.random.default_rng(23)
+    want = mixed_flags(n, 24)
+    x, y, z = rng.uniform(-2, 2, n), rng.uniform(-2, 2, n), rng.uniform(0.5, 5, n)
+    x = np.where(want, 0.1 * x, 2 * z + np.abs(x) + 0.1)
+    y = np.where(want, 0.1 * y, y)
+    xyz = torch.from_numpy(np.stack([x, y, z], -1).astype(np.float32)).to(dev)
+    full_proj = torch.zeros(4, 4)      # [x y z 1] @ M = (x, y, 0.1 z, z): in range iff |x| < 1.1 z and |y| < 1.1 z
+    full_proj[0, 0], full_proj[1, 1], full_proj[2, 2], full_proj[2, 3] = 1.0, 1.0, 0.1, 1.0
+    full_proj = full_proj.to(dev)
+    flag = torch.zeros(n, dtype=torch.uint8, device=dev)
+    index = torch.full((n,), -5, dtype=torch.int64, device=dev)
+    result = torch.zeros(_capi.LGR_PREPARE_RESULTS, dtype=torch.int64, device=dev)
+    scratch = torch.empty(_capi.prepare_scratch_ints(n, 0), dtype=torch.int32, device=dev)
+    p = _capi.LgrPrepare()
+    p.num_points, p.xyz_d, p.full_proj_d = n, _ptr(xyz), _ptr(full_proj)
+    p.bound_lo, p.bound_hi = float(np.float32(-1.1)), float(np.float32(1.1))
+    p.num_roots, p.flag_d, p.in_range_d, p.scratch_d, p.result_d = 0, _ptr(flag), _ptr(index), _ptr(scratch), _ptr(result)
+    assert lib.lgr_prepare_cull(ctypes.byref(p), _capi.current_stream(dev)) == 0
+    assert np.array_equal(flag.cpu().numpy().astype(bool), want)
+    ids = np.nonzero(want)[0]
+    assert int(result[_capi.LGR_PREPARE_IN_RANGE]) == ids.size
+    assert np.array_equal(index[:ids.size].cpu().numpy(), ids)
+
+
+def check_densify_plan(lib, dev):
+    """The densify plan: kept rows, then split parents, each in row order (flag_remove drops a row, and so does
+    flag_split with remove_split)."""
+    from log_b200 import _capi
+    from log_b200.rasterizer import _ptr
+    n = COMPACT_SLOTS
+    rng = np.random.default_rng(25)
+    remove = ~mixed_flags(n, 26)
+    split = rng.random(n) < 0.3
+    st = _capi.current_stream(dev)
+    for remove_split in (0, 1):
+        result = torch.zeros(_capi.LGR_DENSIFY_RESULTS, dtype=torch.int64, device=dev)
+        scratch = torch.empty(_capi.densify_scratch_ints(n), dtype=torch.int32, device=dev)
+        sd, rd = (torch.from_numpy(a.astype(np.uint8)).to(dev) for a in (split, remove))
+        assert lib.lgr_densify_plan(n, _ptr(sd), _ptr(rd), remove_split, _ptr(scratch), _ptr(result), st) == 0
+        keep = np.nonzero(~(remove | (split & bool(remove_split))))[0]
+        parents = np.nonzero(split)[0]
+        res = result.cpu().numpy()
+        assert (res[_capi.LGR_DENSIFY_KEEP], res[_capi.LGR_DENSIFY_SPLIT], res[_capi.LGR_DENSIFY_REMOVED]) == \
+            (keep.size, parents.size, remove.sum())
+        out = torch.full((keep.size + parents.size,), -5, dtype=torch.int64, device=dev)
+        assert lib.lgr_densify_map(n, keep.size, _ptr(scratch), _ptr(out), st) == 0
+        assert np.array_equal(out.cpu().numpy(), np.concatenate([keep, parents]))
+
+
+def check_step_order(lib, dev):
+    """lgr_step_order: the flagged rows ordered by their Gaussian, then -1."""
+    import test_offload
+    n = COMPACT_SLOTS
+    g = torch.Generator().manual_seed(27)
+    perm = torch.randperm(n, generator=g)
+    leaf, node = perm[:n - 20_000].contiguous(), perm[n - 20_000:].contiguous()
+    # flag the row of Gaussian i by mixed_flags[i]: whole empty and full chunks of the Gaussians' scan
+    flag_vis = torch.from_numpy(mixed_flags(n, 28))[perm].to(torch.uint8)
+    order = test_offload._order_via_abi(lib, n, leaf.to(dev), node.to(dev), flag_vis.to(dev))
+    test_offload._check_order(order.cpu(), leaf, node, flag_vis)
+
+
+COMPACTIONS = {'prepare_cull': check_prepare_cull, 'densify_plan': check_densify_plan, 'step_order': check_step_order}
+
+
+@pytest.mark.parametrize('name', list(COMPACTIONS))
+def test_compactions_past_one_scan_pass_emulated(emulated_backend, name):
+    assert -(-COMPACT_SLOTS // COMPACT_CHUNK) > SCAN_PASS, 'case no longer reaches the intended route'
+    COMPACTIONS[name](emulated_backend, device())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('name', list(COMPACTIONS))
+def test_compactions_past_one_scan_pass(built, name):
+    from log_b200 import _capi
+    assert -(-COMPACT_SLOTS // COMPACT_CHUNK) > SCAN_PASS, 'case no longer reaches the intended route'
+    COMPACTIONS[name](_capi.load(), device())
 
 
 # ---- the 10 M-Gaussian, 1080p scene of tests/test_gpu_fullsize.py ------------------------------------------------------
