@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define LGR_ABI_VERSION 27
+#define LGR_ABI_VERSION 28
 #define LGR_TILE 16
 
 /* low-pass filter on the 2D covariance */
@@ -134,6 +134,14 @@ typedef struct lgr_view {
                             dL/dcov3D into dcov3D_d.  Not available with raw_params or in band mode. */
   float* dcov3D_d;       /* (N,6): gradient w.r.t. cov3D_precomp_d (off-diagonal entries receive the sum of the two symmetric
                             partials, like the stock backward); required by lgr_backward when cov3D_precomp_d is set */
+  float* point_depth_d;  /* (n) fp32 or NULL: lgr_forward_project writes the view-space z of each row's mean (LoG's
+                            point_depth, renderer.py:166-168).  Needs gather_index_d and raw_params; written for every row
+                            whose gather entry is >= 0, culled rows included; rows with a negative entry are left as they
+                            were.  NULL: not written. */
+  float* act_rows_d;     /* (n, LGR_ACT_ROW_FLOATS) fp32 or NULL: lgr_forward_project writes each row's activated parameters
+                            (LoG/model/activation.py:27-44): xyz (3), exp(scaling) (3), normalize(rotation) (4),
+                            sigmoid(opacity) (1) and the colour (3), SH2RGB(dc) + eval_sh_wobase(dir, shs, sh_degree),
+                            unclamped, the direction from the mean to campos_d.  Same conditions and rows as point_depth_d. */
   const float* viewmatrix_d; /* (4,4) world_view_transform, stored transposed (LoG/dataset/base.py:40-46) */
   const float* projmatrix_d; /* (4,4) full_proj_transform, same convention */
   const float* campos_d;     /* (3,) */
@@ -143,6 +151,7 @@ typedef struct lgr_view {
 /* Sizes of the buffers the caller must provide. */
 #define LGR_SPLAT_FLOATS 12 /* per-Gaussian projected record: 3 x float4 */
 #define LGR_GRAD_FLOATS 12  /* per-Gaussian 2D-gradient accumulator: 3 x float4 */
+#define LGR_ACT_ROW_FLOATS 14 /* lgr_view.act_rows_d: xyz, scaling, rotation, opacity, colour */
 #define LGR_TILE_SCRATCH_INTS 33 /* per tile: one counter per 128-byte line (32 ints) + one slot of the long-tile list */
 #define LGR_CONTRIB_MAX_LIST (1 << 24) /* longest tile list whose entry indices fit lgr_view.contrib_entry_d */
 #define LGR_META_INTS 8     /* meta_d: [0]=D binned instances [1]=longest tile list [2..3]=D by the stock

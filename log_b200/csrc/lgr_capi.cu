@@ -85,6 +85,8 @@ static bool view_ok(const lgr_view* v) {
   if (v->num_channels != 0 && v->num_channels != 3 && v->num_channels != 6) return false;
   if (v->num_channels == 6 && !v->splat_ext_d) return false;
   if (v->log_depth != 0 && (v->log_depth != 1 || v->num_channels != 6)) return false;      // the depth pass is six channels
+  // LoG's per-row by-products exist for its gathered raw rows only
+  if ((v->point_depth_d || v->act_rows_d) && (!v->gather_index_d || !v->raw_params || v->cov3D_precomp_d)) return false;
   return true;
 }
 

@@ -38,6 +38,23 @@ __device__ __forceinline__ void sh_accumulate(const float* sh, const float B[16]
   }
 }
 
+// The colour of a precomputed (C = RGB) or LoG raw (C = LOG_SH) row: with raw_params SH2RGB(dc) (sh_utils.py:72-73), and
+// for LOG_SH + eval_sh_wobase (sh_utils.py:31-58), basis functions 1 .. (deg+1)^2 - 1 of the direction from the camera
+template <bool LOG_SH>
+__device__ __forceinline__ void row_colour(const View& v, const float* colors, const float* shs, int64_t src, const float p[3],
+                                           const float* cam, float rgb[3]) {
+  load3(colors, src, rgb);
+  if (v.raw_params) {
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) rgb[ch] = fmaf(SH_C0, rgb[ch], 0.5f);
+  }
+  if (LOG_SH && v.sh_degree > 0) {
+    float B[16];
+    sh_dir_basis(p, cam, v.sh_degree, B);
+    sh_accumulate(shs + src * v.sh_K * 3, B, 1, (v.sh_degree + 1) * (v.sh_degree + 1), rgb);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // markVisible of the stock module (diff_gaussian_rasterization's GaussianRasterizer.markVisible): a point is visible
 // when its view-space depth exceeds the near plane -- the same cull the projection applies (NEAR_Z)
@@ -86,6 +103,9 @@ compute_radius_kernel(int64_t n, const float* __restrict__ means, const float* _
 // DEPTH (View::log_depth): channels 3..5 are LoG's depth-pass colours (renderer.py:186-201), generated here for any colour
 // source: (view depth, world z, 1) -> View::splat_ext as (t_z, p_z, 1, 0); t_z is the unclamped view-space z of the mean
 // (cov2d's t[2], record float 11).
+// View::point_depth / View::act_rows (gather + raw_params, checked by the caller): LoG's per-row by-products, the view z of
+// the mean and the activated row (xyz, exp scaling, normalised rotation, sigmoid opacity, colour), written BEFORE the cull
+// because LoG computes them for every gathered row.
 template <Colour C, bool COV3D, bool DEPTH>
 __global__ void __launch_bounds__(PROJ_THREADS)
 project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const float* __restrict__ opac,
@@ -181,6 +201,11 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
         for (int k = 0; k < 3; k++) s[k] = expf(s[k]);
         q = act_normalize(q, inv);
       }
+      if (v.act_rows) {
+        float* a = v.act_rows + (int64_t)LGR_ACT_ROW_FLOATS * i;
+        a[0] = p[0]; a[1] = p[1]; a[2] = p[2]; a[3] = s[0]; a[4] = s[1]; a[5] = s[2];
+        a[6] = q.x; a[7] = q.y; a[8] = q.z; a[9] = q.w;
+      }
 #pragma unroll
       for (int k = 0; k < 3; k++) s[k] *= v.scale_mod;
       quat_to_R(q, R);
@@ -188,6 +213,14 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
     }
     Cov2D cv;
     cov2d(sV, p, Sg, v.fx, v.fy, v.tanfovx, v.tanfovy, v.filter_mode, cv);
+    if (v.point_depth) v.point_depth[i] = cv.t[2];
+    float rgb[3];
+    const bool act = !USE_SH && !SIX && v.act_rows;      // the colour is computed here, once, for the visible branch too
+    if (act) {
+      row_colour<LOG_SH>(v, colors, shs, src, p, sCam, rgb);
+      float* a = v.act_rows + (int64_t)LGR_ACT_ROW_FLOATS * i;
+      a[10] = act_sigmoid(__ldg(opac + src)); a[11] = rgb[0]; a[12] = rgb[1]; a[13] = rgb[2];
+    }
     float det;
     const float radf = radius_from_cov(cv.a, cv.b, cv.c, det);
     float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0, r2 = r0, r3 = r0;
@@ -215,7 +248,6 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
           hx = sqrtf(q * cv.a) * 1.001f + 1e-3f;
           hy = sqrtf(q * cv.c) * 1.001f + 1e-3f;
         }
-        float rgb[3];
         if (USE_SH) {
           float B[16];
           sh_dir_basis(p, sCam, v.sh_degree, B);
@@ -229,17 +261,8 @@ project_fwd_kernel(View v, int64_t n, const float* __restrict__ means, const flo
           const float* c6 = colors + 6 * src;
           rgb[0] = __ldg(c6); rgb[1] = __ldg(c6 + 1); rgb[2] = __ldg(c6 + 2);
           r3 = make_float4(__ldg(c6 + 3), __ldg(c6 + 4), __ldg(c6 + 5), 0.f);
-        } else {
-          load3(colors, src, rgb);
-          if (v.raw_params) {      // SH2RGB (sh_utils.py:72-73)
-#pragma unroll
-            for (int ch = 0; ch < 3; ch++) rgb[ch] = fmaf(SH_C0, rgb[ch], 0.5f);
-          }
-          if (LOG_SH && v.sh_degree > 0) {      // + eval_sh_wobase (sh_utils.py:31-58): basis functions 1 .. (deg+1)^2 - 1
-            float B[16];
-            sh_dir_basis(p, sCam, v.sh_degree, B);
-            sh_accumulate(shs + src * v.sh_K * 3, B, 1, (v.sh_degree + 1) * (v.sh_degree + 1), rgb);
-          }
+        } else if (!act) {
+          row_colour<LOG_SH>(v, colors, shs, src, p, sCam, rgb);
         }
         // conic pre-multiplied by log2(e): the blend evaluates alpha = o * 2^(-0.5 d^T C' d)
         const float kdet = LOG2E * idet;

@@ -75,7 +75,7 @@ def _stream(device=None):
 def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: bool, sh_coeffs: int, tile_rows, keep,
                num_owners=0, band_ids=None, band_count=None, band_blk=None, band_rows=None, band_dsplat=None,
                raw_params=False, gather_index=None, pid_map=None, cov3D_precomp=None, splat_ext=None,
-               log_depth=False):
+               log_depth=False, point_depth=None, act_rows=None):
     dev = s.viewmatrix.device
     vm, pm = _f32c(s.viewmatrix, 'viewmatrix'), _f32c(s.projmatrix, 'projmatrix', dev)
     bg = _f32c(s.bg, 'bg', dev)
@@ -101,6 +101,8 @@ def _make_view(s: GaussianRasterizationSettings, filter_mode: int, want_aux: boo
     if splat_ext is not None:      # six colour channels: channels 3..5 of every projected record live in splat_ext (N,4)
         v.num_channels, v.splat_ext_d = 6, splat_ext.data_ptr()
         v.log_depth = int(bool(log_depth))      # ... generated by the projection as LoG's (view depth, world z, 1)
+    v.point_depth_d = point_depth.data_ptr() if point_depth is not None else None
+    v.act_rows_d = act_rows.data_ptr() if act_rows is not None else None
     v.viewmatrix_d, v.projmatrix_d = vm.data_ptr(), pm.data_ptr()
     v.campos_d = cp.data_ptr() if cp is not None else None
     v.bg_d = bg.data_ptr()
@@ -281,7 +283,7 @@ class RasterState:
 
 def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_precomp, shs, filter_mode, want_aux,
                       tile_rows=None, num_owners=0, raw_params=False, gather_index=None, instance_capacity=None,
-                      cov3D_precomp=None, log_depth=False):
+                      cov3D_precomp=None, log_depth=False, point_depth=None, act_rows=None):
     """Run the forward through the C ABI.  Returns (image, radii, pid, pwp, point_weight, state).
     num_owners > 0 (multi-GPU band mode, see log_b200/sharded.py): also compact the ids of the Gaussians reaching the
     band `tile_rows`, grouped by owner rank; the backward then returns packed gradient rows instead of dense tensors.
@@ -297,7 +299,10 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
     (6,H,W): channels 0..2 equal the call without log_depth bit for bit, channels 3..5 are LoG's depth, height and accmap,
     i.e. the colours (view depth of the mean, world z of the mean, 1) composited over bg[:3].  colors_precomp stays (N,3)
     (or None with shs) and so does its gradient; the height's gradient goes to means3D z, the depth's is dropped (LoG
-    computes it from the detached mean).  Not available in band mode."""
+    computes it from the detached mean).  Not available in band mode.
+    point_depth (M,) / act_rows (M, LGR_ACT_ROW_FLOATS), gather_index with raw_params only: contiguous fp32 outputs the
+    projection fills with LoG's point_depth and activated rows (lgr_view.point_depth_d / act_rows_d) for every row whose
+    gather entry is >= 0, culled rows included."""
     channels = colour_channels(colors_precomp, settings, shs, raw_params, gather_index, num_owners, log_depth)
     if log_depth:      # the blend composites channels 3..5 over bg[3:6]: LoG's second call uses the same background
         bg3 = settings.bg.reshape(-1)[:3]
@@ -334,8 +339,17 @@ def rasterize_forward(settings, means3D, opacities, scales, rotations, colors_pr
         keep.extend([band_ids, band_blk, band_rows, band_count])
     splat_ext = torch.empty((max(n, 1), 4), **f32) if channels == 6 else None      # never NULL
     keep.append(splat_ext)
+    for name, t, width in (('point_depth', point_depth, None), ('act_rows', act_rows, _capi.LGR_ACT_ROW_FLOATS)):
+        if t is None:
+            continue
+        if gather_index is None or not raw_params:
+            raise _capi.LgrError(f'{name} is written for gathered raw rows only (gather_index with raw_params)')
+        want = (n,) if width is None else (n, width)
+        if t.dtype != torch.float32 or tuple(t.shape) != want or not t.is_contiguous() or t.device != dev:
+            raise _capi.LgrError(f'{name} must be a contiguous float32 {want} tensor on {dev}')
     view = _make_view(settings, filter_mode, want_aux, K, tile_rows, keep, num_owners, band_ids, band_count, band_blk, band_rows, band_dsplat,
-                      raw_params, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext, log_depth=log_depth)
+                      raw_params, gather_index, cov3D_precomp=cov3D_precomp, splat_ext=splat_ext, log_depth=log_depth,
+                      point_depth=point_depth, act_rows=act_rows)
     alloc = _fresh(dev)
     splat, radii, clamped, tile_start, tile_cursor, meta = project(view, n, alloc, means3D, opacities, scales, rotations,
                                                                    colors_precomp, shs)
